@@ -176,6 +176,56 @@ __device__ __forceinline__ void wg_mma_chunks(float (&acc)[NC][8], int c0, int n
         if (c >= c0 && c < c0 + nc) wg_mma16(acc[c], ad, wg_desc_sw128(b_addr + (uint32_t)(c - c0) * 2048u));
 }
 
+// acc[0..NC) (+)= A[64 rows at a_addr, K=16] x B[16*NC rows at b_addr, K=16]^T as ONE wgmma m64n(16*NC)k16.  The m64nN
+// accumulator fragment is the n16 fragments of its 16-column chunks concatenated in register order (frag_row / frag_col
+// hold per chunk), and the B rows are contiguous 1024-byte swizzle atoms, so this computes what wg_mma_chunks<NC>(acc,
+// 0, NC, ...) does with one A read instead of NC.  accumulate = 0 overwrites acc with the product (scale-d = 0): the
+// accumulators then need no zeroing by ordinary instructions, which would make ptxas fence (and serialise) the wgmma
+// issue when it sits on a data-dependent path.
+template <int NC> __device__ __forceinline__ void wg_mma_n(float (&acc)[NC][8], uint32_t a_addr, uint32_t b_addr, int accumulate = 1);
+template <> __device__ __forceinline__ void wg_mma_n<1>(float (&d)[1][8], uint32_t a_addr, uint32_t b_addr, int accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0][0]), "+f"(d[0][1]), "+f"(d[0][2]), "+f"(d[0][3]), "+f"(d[0][4]), "+f"(d[0][5]), "+f"(d[0][6]), "+f"(d[0][7])
+        : "l"(wg_desc_sw128(a_addr)), "l"(wg_desc_sw128(b_addr)), "r"(accumulate)
+        : "memory");
+}
+template <> __device__ __forceinline__ void wg_mma_n<2>(float (&d)[2][8], uint32_t a_addr, uint32_t b_addr, int accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0][0]), "+f"(d[0][1]), "+f"(d[0][2]), "+f"(d[0][3]), "+f"(d[0][4]), "+f"(d[0][5]), "+f"(d[0][6]), "+f"(d[0][7]),
+          "+f"(d[1][0]), "+f"(d[1][1]), "+f"(d[1][2]), "+f"(d[1][3]), "+f"(d[1][4]), "+f"(d[1][5]), "+f"(d[1][6]), "+f"(d[1][7])
+        : "l"(wg_desc_sw128(a_addr)), "l"(wg_desc_sw128(b_addr)), "r"(accumulate)
+        : "memory");
+}
+template <> __device__ __forceinline__ void wg_mma_n<3>(float (&d)[3][8], uint32_t a_addr, uint32_t b_addr, int accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, %24, %25, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0][0]), "+f"(d[0][1]), "+f"(d[0][2]), "+f"(d[0][3]), "+f"(d[0][4]), "+f"(d[0][5]), "+f"(d[0][6]), "+f"(d[0][7]),
+          "+f"(d[1][0]), "+f"(d[1][1]), "+f"(d[1][2]), "+f"(d[1][3]), "+f"(d[1][4]), "+f"(d[1][5]), "+f"(d[1][6]), "+f"(d[1][7]),
+          "+f"(d[2][0]), "+f"(d[2][1]), "+f"(d[2][2]), "+f"(d[2][3]), "+f"(d[2][4]), "+f"(d[2][5]), "+f"(d[2][6]), "+f"(d[2][7])
+        : "l"(wg_desc_sw128(a_addr)), "l"(wg_desc_sw128(b_addr)), "r"(accumulate)
+        : "memory");
+}
+template <> __device__ __forceinline__ void wg_mma_n<4>(float (&d)[4][8], uint32_t a_addr, uint32_t b_addr, int accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,"
+        "%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0][0]), "+f"(d[0][1]), "+f"(d[0][2]), "+f"(d[0][3]), "+f"(d[0][4]), "+f"(d[0][5]), "+f"(d[0][6]), "+f"(d[0][7]),
+          "+f"(d[1][0]), "+f"(d[1][1]), "+f"(d[1][2]), "+f"(d[1][3]), "+f"(d[1][4]), "+f"(d[1][5]), "+f"(d[1][6]), "+f"(d[1][7]),
+          "+f"(d[2][0]), "+f"(d[2][1]), "+f"(d[2][2]), "+f"(d[2][3]), "+f"(d[2][4]), "+f"(d[2][5]), "+f"(d[2][6]), "+f"(d[2][7]),
+          "+f"(d[3][0]), "+f"(d[3][1]), "+f"(d[3][2]), "+f"(d[3][3]), "+f"(d[3][4]), "+f"(d[3][5]), "+f"(d[3][6]), "+f"(d[3][7])
+        : "l"(wg_desc_sw128(a_addr)), "l"(wg_desc_sw128(b_addr)), "r"(accumulate)
+        : "memory");
+}
+
 // Accumulator fragment of m64n16 per thread (warp w = warp % 4 of the warpgroup): value pair i (0..3) of chunk c is
 // acc[c][2i], acc[c][2i+1] at row 16w + lane/4 + 8*(i&1), columns 16c + 8*(i>>1) + 2*(lane&3) + {0,1}.
 __device__ __forceinline__ int frag_row(int wq, int lane, int i) { return 16 * wq + (lane >> 2) + 8 * (i & 1); }

@@ -70,8 +70,10 @@ struct BkParams {
 };
 
 // STREAM = 0: all weights of the block resident in shared memory; STREAM = 1: expansion / depthwise / projection weights
-// travel through two-slot rings (blocks with Ce up to 288 at Cin = 48: stage 2 of LitePose-S)
-template <int STREAM>
+// travel through two-slot rings (blocks with Ce up to 288 at Cin = 48: stage 2 of LitePose-S).
+// K16 = ceil(Cin / 16) K=16 steps of the expansion, NC = n_tile / 16 projection chunks: compile-time widths, so that every
+// wgmma is issued straight-line (one m64n32k16 per expansion slice, one m64n(16 NC)k16 per projection slice).
+template <int STREAM, int K16, int NC>
 __global__ void __launch_bounds__(BK_THREADS, 1)
 block_s1_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_we,
                 const __grid_constant__ CUtensorMap map_dw, const __grid_constant__ CUtensorMap map_wp,
@@ -113,6 +115,11 @@ block_s1_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
         sBdw[i] = (i < p.Ce && p.b_dw) ? p.b_dw[i] : 0.f;
     }
     for (int i = threadIdx.x; i < p.n_tile; i += BK_THREADS) sBpj[i] = p.b_pj ? p.b_pj[i] : 0.f;
+    // The projection always runs all four K=16 slices of a K block.  In the half K block of an odd slab count the A
+    // channels 32..63 hold zeros (or the ReLU6 outputs of an earlier K block) against zero-padded weights: exact zero
+    // products, which leave the fp32 accumulators unchanged.
+    for (int i = threadIdx.x; i < 2 * BK_A_TILE / 16; i += BK_THREADS) reinterpret_cast<uint4*>(sA)[i] = make_uint4(0, 0, 0, 0);
+    fence_proxy_async();
     pdl_launch_dependents();
     __syncthreads();
 
@@ -185,12 +192,11 @@ block_s1_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
         const int by = blk >> 2, bx = blk & 3;
         const int oy = by * 4, ox = bx * 4;
         uint8_t* slab = sSlab + grp * BK_SLAB;
-        const int nch = p.n_tile >> 4;
         const uint32_t a_wg = smem_u32(sA + (wg >> 1) * BK_A_TILE) + (wg & 1) * 8192;
         const __half2 zero2 = __floats2half2_rn(0.f, 0.f), six2 = __floats2half2_rn(6.f, 6.f);
         uint32_t ec = 0;                                   // slabs expanded by this group
         int it = 0;
-        float pacc[4][8];                                  // projection accumulators, n_tile <= 64
+        float pacc[NC][8];                                 // projection accumulators
         if (!STREAM) mbar_wait(&bars->w_full, 0);           // weights resident
         pdl_wait();                                        // the identity rows are read from global memory
         for (int t = blockIdx.x; t < p.num_tiles; t += gridDim.x, ++it) {
@@ -206,9 +212,21 @@ block_s1_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
                 if (lane == 0) mbar_arrive(&bars->x_empty);
             }
 #pragma unroll
-            for (int c = 0; c < 4; ++c)
+            for (int c = 0; c < NC; ++c)
 #pragma unroll
                 for (int i = 0; i < 8; ++i) pacc[c][i] = 0.f;
+            // which of the thread's 8 haloed pixels (expansion rows (ewg * 4 + j) * 64 + frag_row(wq, lane, 0 / 1), j = 0..3)
+            // lie inside the image: the same for every slab of the tile
+            uint32_t in_img = 0;
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    const int pi = (ewg * 4 + j) * 64 + frag_row(wq, lane, i);
+                    const int yy = pi / BK_I, xx = pi - yy * BK_I;
+                    const int gy = ty * BK_T - 3 + yy, gx = tx * BK_T - 3 + xx;
+                    if (pi < BK_PIX && gy >= 0 && gy < p.H && gx >= 0 && gx < p.W) in_img |= 1u << (j * 2 + i);
+                }
             for (int kb = 0; kb < p.nkb; ++kb) {
                 const int s = 2 * kb + vg;
                 const bool have = s < p.nslabs;
@@ -235,19 +253,13 @@ block_s1_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
                         }
 #pragma unroll
                     for (int hb = 0; hb < 2; ++hb) {
-                        float eacc[2][2][8];
-#pragma unroll
-                        for (int b = 0; b < 2; ++b)
-#pragma unroll
-                            for (int c = 0; c < 2; ++c)
-#pragma unroll
-                                for (int i = 0; i < 8; ++i) eacc[b][c][i] = 0.f;
+                        float eacc[2][2][8];                 // written by the first K=16 slice (scale-d = 0)
                         const uint32_t x_base = smem_u32(sX) + (ewg * 4 + hb * 2) * 8192;
                         wg_fence();
 #pragma unroll
                         for (int b = 0; b < 2; ++b)
-                            for (int k = 0; k < p.k16; ++k)
-                                wg_mma_chunks<2>(eacc[b], 0, 2, x_base + b * 8192 + k * 32, b_base + k * 32);
+#pragma unroll
+                            for (int k = 0; k < K16; ++k) wg_mma_n<2>(eacc[b], x_base + b * 8192 + k * 32, b_base + k * 32, k);
                         wg_commit();
                         wg_wait0();
                         // + bias in fp32, round to fp16, ReLU6 on the packed halves (clamping commutes with rounding),
@@ -258,9 +270,7 @@ block_s1_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
                             for (int i = 0; i < 4; ++i) {
                                 const int pi = (ewg * 4 + hb * 2 + b) * 64 + frag_row(wq, lane, i);
                                 if (pi >= BK_PIX) continue;
-                                const int yy = pi / BK_I, xx = pi - yy * BK_I;
-                                const int gy = ty * BK_T - 3 + yy, gx = tx * BK_T - 3 + xx;
-                                const bool in = gy >= 0 && gy < p.H && gx >= 0 && gx < p.W;
+                                const bool in = (in_img >> ((hb * 2 + b) * 2 + (i & 1))) & 1;
 #pragma unroll
                                 for (int c = 0; c < 2; ++c) {
                                     const int ch = c * 16 + frag_col(lane, i);
@@ -306,7 +316,6 @@ block_s1_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
                 }
                 asm volatile("bar.sync 3, 512;" ::: "memory");                  // A tile complete
                 // ---- projection of K block kb
-                const int k16 = 2 * min(2, p.nslabs - 2 * kb);
                 const uint32_t wp_i = (uint32_t)(it * p.nkb + kb);
                 uint32_t b_base = smem_u32(sWp + kb * p.n_tile * 128);
                 if (STREAM) {
@@ -314,7 +323,8 @@ block_s1_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
                     b_base = smem_u32(sWp + (wp_i & 1) * p.wp_stage);
                 }
                 wg_fence();
-                for (int k = 0; k < k16; ++k) wg_mma_chunks<4>(pacc, 0, nch, a_wg + k * 32, b_base + k * 32);
+#pragma unroll
+                for (int k = 0; k < 4; ++k) wg_mma_n<NC>(pacc, a_wg + k * 32, b_base + k * 32);
                 wg_commit();
                 wg_wait0();
                 if (STREAM) {
@@ -331,9 +341,9 @@ block_s1_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
                 if (gy >= p.H || gx >= p.W) continue;
                 const size_t off = (((size_t)n * p.H + gy) * p.W + gx) * p.Co;
 #pragma unroll
-                for (int c = 0; c < 4; ++c) {
+                for (int c = 0; c < NC; ++c) {
                     const int co = c * 16 + frag_col(lane, i);
-                    if (c >= nch || co >= p.Co) continue;
+                    if (co >= p.Co) continue;
                     float2 v = make_float2(pacc[c][2 * i] + sBpj[co], pacc[c][2 * i + 1] + sBpj[co + 1]);
                     if (p.residual) {
                         const float2 f = __half22float2(*reinterpret_cast<const __half2*>(p.residual + off + co));
@@ -457,17 +467,24 @@ extern "C" int lp_block_s1_f16(const void* x, const void* w_exp_packed, const fl
         if (rc) return rc;
     }
     const int grid = p.num_tiles < num_sms() ? p.num_tiles : num_sms();
-    cudaError_t e, le;
-    if (stream_mode) {
-        e = cudaFuncSetAttribute((const void*)block_s1_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, need);
-        if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(block_s1)");
-        le = launch_pdl(block_s1_kernel<1>, dim3(grid), dim3(BK_THREADS), (size_t)need, (cudaStream_t)stream, mx, mwe, mdw, mwp, p);
-    } else {
-        e = cudaFuncSetAttribute((const void*)block_s1_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, need);
-        if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(block_s1)");
-        le = launch_pdl(block_s1_kernel<0>, dim3(grid), dim3(BK_THREADS), (size_t)need, (cudaStream_t)stream, mx, mwe, mdw, mwp, p);
-    }
-    if (le != cudaSuccess) return cuda_fail(le, "launch block_s1_kernel");
+    const int nc = p.n_tile / 16;
+    using Kern = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const BkParams);
+    // [layout][k16 - 1][nc - 1]
+    static const Kern kernels[2][4][4] = {
+        {{block_s1_kernel<0, 1, 1>, block_s1_kernel<0, 1, 2>, block_s1_kernel<0, 1, 3>, block_s1_kernel<0, 1, 4>},
+         {block_s1_kernel<0, 2, 1>, block_s1_kernel<0, 2, 2>, block_s1_kernel<0, 2, 3>, block_s1_kernel<0, 2, 4>},
+         {block_s1_kernel<0, 3, 1>, block_s1_kernel<0, 3, 2>, block_s1_kernel<0, 3, 3>, block_s1_kernel<0, 3, 4>},
+         {block_s1_kernel<0, 4, 1>, block_s1_kernel<0, 4, 2>, block_s1_kernel<0, 4, 3>, block_s1_kernel<0, 4, 4>}},
+        {{block_s1_kernel<1, 1, 1>, block_s1_kernel<1, 1, 2>, block_s1_kernel<1, 1, 3>, block_s1_kernel<1, 1, 4>},
+         {block_s1_kernel<1, 2, 1>, block_s1_kernel<1, 2, 2>, block_s1_kernel<1, 2, 3>, block_s1_kernel<1, 2, 4>},
+         {block_s1_kernel<1, 3, 1>, block_s1_kernel<1, 3, 2>, block_s1_kernel<1, 3, 3>, block_s1_kernel<1, 3, 4>},
+         {block_s1_kernel<1, 4, 1>, block_s1_kernel<1, 4, 2>, block_s1_kernel<1, 4, 3>, block_s1_kernel<1, 4, 4>}},
+    };
+    const Kern k = kernels[stream_mode][p.k16 - 1][nc - 1];
+    cudaError_t e = cudaFuncSetAttribute((const void*)k, cudaFuncAttributeMaxDynamicSharedMemorySize, need);
+    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(block_s1)");
+    e = launch_pdl(k, dim3(grid), dim3(BK_THREADS), (size_t)need, (cudaStream_t)stream, mx, mwe, mdw, mwp, p);
+    if (e != cudaSuccess) return cuda_fail(e, "launch block_s1_kernel");
     LP_LAUNCH_CHECK("block_s1_kernel");
     return LP_OK;
 }

@@ -1,12 +1,17 @@
-"""Times the block-level kernels at the stage shapes of LitePose-S @512 batch 32 (CUDA events, L2 flushed):
-fused block kernel vs expansion GEMM + fused depthwise/projection kernel."""
-import os, sys, json
+"""Times the block-level kernels at the three stage shapes of LitePose-S @512 (CUDA events, L2 flushed), by default at
+batch 64 (a batch-32 step runs the plain and the mirrored pass concurrently on two streams, about the work of one
+batch-64 launch): fused block kernel vs expansion GEMM + fused depthwise/projection kernel.  dw_tmacs is the fused
+block's depthwise work (N*H*W*Ce*49 MAC) over its time."""
+import os, sys, json, argparse, subprocess
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
 from litepose_b200 import _lib
 lib = _lib.load()
 dev = torch.device("cuda", 0)
 flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
+ap = argparse.ArgumentParser()
+ap.add_argument("--batch", type=int, default=64)
+args = ap.parse_args()
 
 def timeit(fn, iters=12, skip=3):
     ts = []
@@ -25,7 +30,8 @@ def pack_pw(w, K, N):
 
 out = {}
 s = torch.cuda.current_stream().cuda_stream
-for (n, hw, cin, ce, co) in ((32, 128, 16, 96, 16), (32, 64, 32, 192, 32)):
+for (hw, cin, ce, co) in ((128, 16, 96, 16), (64, 32, 192, 32), (32, 48, 288, 48)):
+    n = args.batch
     rs = np.random.RandomState(0)
     x = torch.randn((n, hw, hw, cin), device=dev).half()
     we = (rs.randn(ce, cin) / cin ** 0.5).astype(np.float32)
@@ -44,5 +50,11 @@ for (n, hw, cin, ce, co) in ((32, 128, 16, 96, 16), (32, 64, 32, 192, 32)):
     t_exp = timeit(lambda: _lib.check(lib.lp_pw1x1_f16(x.data_ptr(), wexp.data_ptr(), bexp.data_ptr(), None, e.data_ptr(), n * hw * hw, cin, ce, 2, s)))
     t_dwp = timeit(lambda: _lib.check(lib.lp_dw7_project_f16(e.data_ptr(), wd.data_ptr(), bd.data_ptr(), wpd.data_ptr(), bpd.data_ptr(),
                                                               x.data_ptr(), o.data_ptr(), n, hw, hw, ce, co, s)))
-    out["%dx%dx%dx%d->%d->%d" % (n, hw, hw, cin, ce, co)] = {"block_us": t_blk, "expand_us": t_exp, "dw_project_us": t_dwp}
-print(json.dumps({"skew_ns": os.environ.get("LP_BLOCK_SKEW_NS", "0"), "shapes": out}))
+    out["%dx%dx%dx%d->%d->%d" % (n, hw, hw, cin, ce, co)] = {"block_us": t_blk, "expand_us": t_exp, "dw_project_us": t_dwp,
+                                                              "dw_tmacs": n * hw * hw * ce * 49 / t_blk / 1e6}
+try:
+    r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
+    gpu = r.stdout.strip().splitlines()[0]
+except Exception:
+    gpu = torch.cuda.get_device_name(0)
+print(json.dumps({"gpu": gpu, "skew_ns": os.environ.get("LP_BLOCK_SKEW_NS", "0"), "shapes": out}))
