@@ -2,7 +2,8 @@
 // (reference lib/models/layers/layers.py:100-118: depth_conv -> point_conv -> optional identity add).
 //
 // Unfused, the 6x-expanded tensor is written by the depthwise kernel and read back by the projection GEMM; here it
-// never leaves the SM.  Per CTA (persistent over 16x16-pixel output tiles):
+// never leaves the SM.  Projections up to 64 channels (and the heads) run dw_project_kernel; wider block projections run
+// dw_project_wide_kernel further below.  dw_project_kernel, per CTA (persistent over 16x16-pixel output tiles):
 //   warp 16 (1 thread) TMA producer: haloed 22x22x32-channel input slabs (hardware zero fill = conv padding) into a
 //                      4-deep ring, projection-weight K blocks into a 2-deep ring
 //   warps 0-15         depthwise on the CUDA cores, two groups of 8 warps working on the two 32-channel halves of a
@@ -16,6 +17,7 @@
 // HBM traffic per block: read N*H*W*Ce*2 (+ N*H*W*Co*2 residual), write N*H*W*Co*2  -- the depthwise output
 // (N*H*W*Ce*2 written + read again) is gone; the kernel is bound by the FMA pipe (2*49 flop per expanded element).
 #include "common.cuh"
+#include "dw_inner.cuh"
 
 namespace lp {
 
@@ -36,7 +38,7 @@ constexpr int FP_B_BYTES = 160 * 64 * 2;                      // Co <= 160
 constexpr int FP_DW_WARPS = 16;                                // two groups of 8: even / odd 32-channel slabs
 constexpr int FP_THREADS = (FP_DW_WARPS + 4) * 32;   // + one producer warpgroup (one thread of it works)
 // registers: 20 warps leave 96 per thread at launch (5 warps per SM sub-partition); the producer warpgroup gives up
-// 72 of them so that the four compute warpgroups, which hold up to 80 accumulators each, run with 112
+// 72 of them so that the four compute warpgroups, which hold up to 64 accumulators each, run with 112
 constexpr int FP_REGS_PRODUCER = 24, FP_REGS_COMPUTE = 112;
 // setmaxnreg.inc only draws on what setmaxnreg.dec released in the CTA: 128 x (96 - 24) >= 512 x (112 - 96)
 static_assert(128 * (96 - FP_REGS_PRODUCER) >= 512 * (FP_REGS_COMPUTE - 96), "register hand-over exceeds the released pool");
@@ -331,12 +333,230 @@ template <int K, int HEAD>
 static int launch_dw_project(const CUtensorMap& m0, const CUtensorMap& m1, const CUtensorMap& mw, const CUtensorMap& md,
                              const FpParams& p, cudaStream_t stream) {
     if (p.n_tile <= 32) return launch_dw_project_nc<K, HEAD, 2>(m0, m1, mw, md, p, stream);
-    if (p.n_tile <= 64) return launch_dw_project_nc<K, HEAD, 4>(m0, m1, mw, md, p, stream);
-    if constexpr (HEAD) {
-        return launch_dw_project_nc<K, HEAD, 8>(m0, m1, mw, md, p, stream);     // heads: Co <= 128
+    if constexpr (!HEAD) {
+        return launch_dw_project_nc<K, HEAD, 4>(m0, m1, mw, md, p, stream);     // blocks: Co <= 64 (wider: below)
     } else {
-        if (p.n_tile <= 128) return launch_dw_project_nc<K, HEAD, 8>(m0, m1, mw, md, p, stream);
-        return launch_dw_project_nc<K, HEAD, 10>(m0, m1, mw, md, p, stream);
+        if (p.n_tile <= 64) return launch_dw_project_nc<K, HEAD, 4>(m0, m1, mw, md, p, stream);
+        return launch_dw_project_nc<K, HEAD, 8>(m0, m1, mw, md, p, stream);     // heads: Co <= 128
+    }
+}
+
+// ------------------------------------------------------------------ wide projections (block Co 65..160)
+// dw_project_kernel keeps its projection accumulators live through the depthwise loop; at Co > 64 they no longer fit
+// beside the loop's ~95 registers and ptxas spills inside it.  This kernel gives the two jobs to different warps:
+//   warps 0-7   (2 warpgroups) depthwise, two groups of 4 warps on the even / odd 32-channel slabs of a K block: one
+//               4x4 micro-block x channel pair per thread (dw_inner.cuh, the same packed-fp16 chain as above), ReLU6'd
+//               fp16 results into a 2-deep ring of 128B-swizzled A tiles (full / empty mbarriers)
+//   warps 8-15  (2 warpgroups) projection: wgmma m64 x n(16 NC) x k16 over 64 pixels each, fp32 accumulators in
+//               registers; every K block is committed and the previous one waited for (wait_group 1), so the MMAs of
+//               K block kb run under the depthwise of kb + 1; then the bias / residual / NHWC epilogue, which runs
+//               under the depthwise of the next tile
+// There is no producer warp: the first thread of each depthwise group issues the TMA loads of its group's haloed
+// 22x14x32 input slabs + depthwise weights (two ring stages per group, the slab after next is loaded when the slab
+// before is released), the first MMA thread those of the projection-weight K blocks (two-slot ring).  ptxas compiles
+// a kernel for one register budget, whatever setmaxnreg does at run time; with 16 warps that budget is 128, enough for
+// the 80 accumulators of NC = 10 and for the depthwise loop (a 17th warp would count as 20 and leave 96).
+// Tiles are 16 x 8 pixels (one 128-row M-tile): more tiles per persistent CTA than 16 x 16, so that the epilogue and
+// pipeline fill of one tile hide under the next.
+constexpr int FW_TX = 16, FW_TY = 8;                              // output tile
+constexpr int FW_IX = FW_TX + 6, FW_IY = FW_TY + 6;               // haloed input slab: 22 x 14 pixels
+constexpr int FW_IN_BYTES = FW_IX * FW_IY * FP_CB * 2;            // 19712
+constexpr int FW_W_OFF = FW_IN_BYTES;                             // depthwise weights of the slab (128-byte aligned)
+constexpr int FW_IN_STRIDE = 23552;                               // ring pitch (multiple of 1024)
+constexpr int FW_NIN = 4;                                         // slab ring: group g uses stages g and g + 2
+constexpr int FW_NA = 2, FW_NB = 2;                               // A-tile ring, projection-weight ring
+constexpr int FW_DW_WARPS = 8, FW_MMA_WARPS = 8;
+constexpr int FW_THREADS = (FW_DW_WARPS + FW_MMA_WARPS) * 32;
+static_assert(FW_W_OFF % 128 == 0 && FW_W_OFF + FpCfg<7>::W_BYTES <= FW_IN_STRIDE, "ring stage layout");
+constexpr size_t FW_SMEM = (size_t)FW_NIN * FW_IN_STRIDE + FW_NA * FP_A_TILE + FW_NB * FP_B_BYTES + 1024 + FP_MAX_CE * 4 + 1024;
+
+struct FwBars {
+    uint64_t in_full[FW_NIN], in_empty[FW_NIN];
+    uint64_t a_full[FW_NA], a_empty[FW_NA];
+    uint64_t b_full[FW_NB], b_empty[FW_NB];
+};
+
+// NC = n_tile / 16 exactly: every K=16 slice of the projection is one straight-line m64n(16 NC)k16.
+template <int NC>
+__global__ void __launch_bounds__(FW_THREADS, 1)
+dw_project_wide_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w,
+                       const __grid_constant__ CUtensorMap map_dw, const __grid_constant__ FpParams p) {
+    extern __shared__ __align__(1024) uint8_t smem[];
+    uint8_t* sIn = smem;                                          // FW_NIN x ([14][22][32] fp16 + [49][32] fp16)
+    uint8_t* sA = smem + FW_NIN * FW_IN_STRIDE;                   // FW_NA x [128 px][64 ch], 128B-swizzled
+    uint8_t* sB = sA + FW_NA * FP_A_TILE;                         // FW_NB x [n_tile][64] fp16, 128B-swizzled
+    float* sBias = reinterpret_cast<float*>(sB + FW_NB * FP_B_BYTES);     // projection bias (<= 160)
+    float* sBdw = sBias + 192;                                             // depthwise bias (<= FP_MAX_CE)
+    FwBars* bars = reinterpret_cast<FwBars*>(sBdw + FP_MAX_CE);
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t my_tiles = (p.num_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x;   // grid <= num_tiles
+
+    if (threadIdx.x == 0) {
+        tma_prefetch_desc(&map_x);
+        tma_prefetch_desc(&map_w);
+        tma_prefetch_desc(&map_dw);
+        for (int i = 0; i < FW_NIN; ++i) { mbar_init(&bars->in_full[i], 1); mbar_init(&bars->in_empty[i], FW_DW_WARPS / 2); }
+        for (int i = 0; i < FW_NA; ++i) { mbar_init(&bars->a_full[i], FW_DW_WARPS); mbar_init(&bars->a_empty[i], FW_MMA_WARPS); }
+        for (int i = 0; i < FW_NB; ++i) { mbar_init(&bars->b_full[i], 1); mbar_init(&bars->b_empty[i], FW_MMA_WARPS); }
+        fence_barrier_init();
+    }
+    for (int i = threadIdx.x; i < p.n_tile; i += FW_THREADS) sBias[i] = p.b_pj ? p.b_pj[i] : 0.f;
+    for (int i = threadIdx.x; i < p.nslabs * FP_CB; i += FW_THREADS) sBdw[i] = (p.b_dw && i < p.Ce) ? p.b_dw[i] : 0.f;
+    // The projection always runs all four K=16 slices of a K block.  In the half K block of an odd slab count the A
+    // channels 32..63 hold zeros (or ReLU6 outputs of an earlier K block) against zero-padded weights: exact zero
+    // products, which leave the fp32 accumulators unchanged.
+    for (int i = threadIdx.x; i < FW_NA * FP_A_TILE / 16; i += FW_THREADS) reinterpret_cast<uint4*>(sA)[i] = make_uint4(0, 0, 0, 0);
+    fence_proxy_async();
+    pdl_launch_dependents();
+    __syncthreads();
+    pdl_wait();                   // the expanded input of this block is complete from here on
+
+    if (warp < FW_DW_WARPS) {
+        // ------------------------------------------------------------------ depthwise warps
+        const int cp = threadIdx.x & 15;
+        const bool mir = ((threadIdx.x >> 4) & 1) != 0;
+        const int grp = warp >> 2;                         // 0: even slabs (channels 0-31 of a K block), 1: odd slabs
+        const int blk = ((warp & 3) << 1) | (int)mir;      // 8 micro-blocks: 2 x 4 of 4x4 pixels
+        const int oy = (blk >> 2) * 4, ox = (blk & 3) * 4;
+        const int jch = (grp << 2) | (cp >> 2);
+        const bool loader = (warp & 3) == 0 && lane == 0;
+        const uint32_t ng = (p.nslabs - grp + 1) >> 1;    // slabs of this group per tile
+        const uint32_t nj = ng * my_tiles;
+        // slab j of this group's sequence (tile j / ng of the CTA, its K block j % ng) -> stage 2 (j & 1) + grp
+        auto load_slab = [&](uint32_t j) {
+            const int t = blockIdx.x + (int)(j / ng) * gridDim.x, s = 2 * (int)(j % ng) + grp;
+            const int tx = t % p.tiles_x, ty = (t / p.tiles_x) % p.tiles_y, n = t / (p.tiles_x * p.tiles_y);
+            const uint32_t is = 2 * (j & 1) + grp;
+            mbar_expect_tx(&bars->in_full[is], FW_IN_BYTES + FpCfg<7>::W_BYTES);
+            tma_load_4d(sIn + is * FW_IN_STRIDE, &map_x, &bars->in_full[is], s * FP_CB, tx * FW_TX - 3, ty * FW_TY - 3, n);
+            tma_load_2d(sIn + is * FW_IN_STRIDE + FW_W_OFF, &map_dw, &bars->in_full[is], s * FP_CB, 0);
+        };
+        if (loader) {
+            if (nj > 0) load_slab(0);
+            if (nj > 1) load_slab(1);
+        }
+        uint32_t iu = 0, au = 0;                           // slabs consumed by this group, K blocks handed over
+        for (int t = blockIdx.x; t < p.num_tiles; t += gridDim.x) {
+            for (int kb = 0; kb < p.nkb; ++kb, ++au) {
+                const int s = 2 * kb + grp;
+                const bool have = s < p.nslabs;            // the last K block may hold a single slab
+                __half2 acch[4][4];
+                if (have) {
+                    const uint32_t is = 2 * (iu & 1) + grp;
+                    if (loader && iu >= 1 && iu + 1 < nj) {
+                        // the other stage of the group: slab iu - 1 is released by all four warps -> slab iu + 1
+                        mbar_wait(&bars->in_empty[is ^ 2], ((iu - 1) >> 1) & 1);
+                        load_slab(iu + 1);
+                    }
+                    const __half2 bh = __float22half2_rn(*reinterpret_cast<const float2*>(sBdw + s * FP_CB + 2 * cp));
+                    mbar_wait(&bars->in_full[is], (iu >> 1) & 1);
+                    const uint8_t* st = sIn + is * FW_IN_STRIDE;
+                    dw_slab_hfma2<7, 4, FW_IX, FP_CB>(reinterpret_cast<const __half2*>(st),
+                                                      reinterpret_cast<const __half2*>(st + FW_W_OFF), cp, mir, oy, ox, bh, acch);
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&bars->in_empty[is]);
+                    ++iu;
+                }
+                const uint32_t q = au & 1;
+                mbar_wait(&bars->a_empty[q], ((au >> 1) & 1) ^ 1);
+                if (have) {
+                    dw_store_a<4>(sA + q * FP_A_TILE, FP_A_TILE, acch, oy, ox, mir, jch, cp);
+                    fence_proxy_async();
+                }
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&bars->a_full[q]);
+            }
+        }
+    } else {
+        // ------------------------------------------------------------------ projection MMAs + epilogue
+        const int wg = (warp - FW_DW_WARPS) >> 2, wq = warp & 3;        // rows 64 wg .. 64 wg + 63 of the tile
+        const bool loader = warp == FW_DW_WARPS && lane == 0;
+        const uint32_t nu = my_tiles * p.nkb;
+        auto load_w = [&](uint32_t v) {                                 // K block v % nkb -> slot v & 1
+            const uint32_t q = v & 1;
+            mbar_expect_tx(&bars->b_full[q], p.n_tile * 128);
+            tma_load_2d(sB + q * FP_B_BYTES, &map_w, &bars->b_full[q], 0, (int)(v % p.nkb) * p.n_tile);
+        };
+        // K block v has retired in this warp: release its A tile and weight slot; the loader refills the slot with v + 2
+        auto release = [&](uint32_t v) {
+            __syncwarp();
+            if (lane == 0) { mbar_arrive(&bars->a_empty[v & 1]); mbar_arrive(&bars->b_empty[v & 1]); }
+            if (loader && v + 2 < nu) {
+                mbar_wait(&bars->b_empty[v & 1], (v >> 1) & 1);
+                load_w(v + 2);
+            }
+        };
+        if (loader) {
+            load_w(0);
+            if (nu > 1) load_w(1);
+        }
+        uint32_t u = 0;                                                 // K blocks consumed (A and B rings alike)
+        float pacc[NC][8];
+        for (int t = blockIdx.x; t < p.num_tiles; t += gridDim.x) {
+            for (int kb = 0; kb < p.nkb; ++kb, ++u) {
+                const uint32_t q = u & 1, ph = (u >> 1) & 1;
+                mbar_wait(&bars->a_full[q], ph);
+                mbar_wait(&bars->b_full[q], ph);
+                const uint32_t a_base = smem_u32(sA + q * FP_A_TILE) + wg * 8192, b_base = smem_u32(sB + q * FP_B_BYTES);
+                wg_fence();
+#pragma unroll
+                for (int k = 0; k < 4; ++k) wg_mma_n<NC>(pacc, a_base + k * 32, b_base + k * 32, kb | k);
+                wg_commit();
+                if (kb > 0) {
+                    wg_wait1();
+                    release(u - 1);
+                }
+            }
+            wg_wait0();
+            release(u - 1);
+            // epilogue: accumulator row = pixel of the 16 x 8 tile
+            const int tx = t % p.tiles_x, ty = (t / p.tiles_x) % p.tiles_y, n = t / (p.tiles_x * p.tiles_y);
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int row = wg * 64 + frag_row(wq, lane, i);
+                const int gy = ty * FW_TY + (row >> 4), gx = tx * FW_TX + (row & 15);
+                if (gy >= p.H || gx >= p.W) continue;
+                const size_t off = (((size_t)n * p.H + gy) * p.W + gx) * p.Co;
+#pragma unroll
+                for (int c = 0; c < NC; ++c) {
+                    const int co = c * 16 + frag_col(lane, i);
+                    if (co >= p.Co) continue;
+                    float2 v = make_float2(pacc[c][2 * i] + sBias[co], pacc[c][2 * i + 1] + sBias[co + 1]);
+                    if (p.residual) {
+                        const float2 f = __half22float2(*reinterpret_cast<const __half2*>(p.residual + off + co));
+                        v.x += f.x;
+                        v.y += f.y;
+                    }
+                    *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(p.out) + off + co) = __float22half2_rn(v);
+                }
+            }
+        }
+    }
+}
+
+template <int NC>
+static int launch_dw_project_wide_nc(const CUtensorMap& mx, const CUtensorMap& mw, const CUtensorMap& md, const FpParams& p,
+                                     cudaStream_t stream) {
+    auto kern = dw_project_wide_kernel<NC>;
+    cudaError_t e = cudaFuncSetAttribute((const void*)kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FW_SMEM);
+    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(dw_project_wide_kernel)");
+    const int grid = p.num_tiles < num_sms() ? p.num_tiles : num_sms();
+    cudaError_t le = launch_pdl(kern, dim3(grid), dim3(FW_THREADS), FW_SMEM, stream, mx, mw, md, p);
+    if (le != cudaSuccess) return cuda_fail(le, "launch dw_project_wide_kernel");
+    LP_LAUNCH_CHECK("dw_project_wide_kernel");
+    return LP_OK;
+}
+
+static int launch_dw_project_wide(const CUtensorMap& mx, const CUtensorMap& mw, const CUtensorMap& md, const FpParams& p,
+                                  cudaStream_t stream) {
+    switch (p.n_tile / 16) {
+        case 5: return launch_dw_project_wide_nc<5>(mx, mw, md, p, stream);
+        case 6: return launch_dw_project_wide_nc<6>(mx, mw, md, p, stream);
+        case 7: return launch_dw_project_wide_nc<7>(mx, mw, md, p, stream);
+        case 8: return launch_dw_project_wide_nc<8>(mx, mw, md, p, stream);
+        case 9: return launch_dw_project_wide_nc<9>(mx, mw, md, p, stream);
+        default: return launch_dw_project_wide_nc<10>(mx, mw, md, p, stream);
     }
 }
 
@@ -363,8 +583,10 @@ extern "C" int lp_dw7_project_f16(const void* x, const void* w_dw, const float* 
     memset(&p, 0, sizeof(p));
     p.N = N; p.H = H; p.W = W; p.Ce = Ce; p.Co = Co;
     p.n_tile = (Co + 15) / 16 * 16;
-    p.tiles_x = (W + FP_T - 1) / FP_T;
-    p.tiles_y = (H + FP_T - 1) / FP_T;
+    const bool wide = p.n_tile > 64;                  // dw_project_wide_kernel, 16 x 8 tiles
+    const int tw = wide ? FW_TX : FP_T, th = wide ? FW_TY : FP_T;
+    p.tiles_x = (W + tw - 1) / tw;
+    p.tiles_y = (H + th - 1) / th;
     p.num_tiles = p.tiles_x * p.tiles_y * N;
     p.nslabs = (Ce + FP_CB - 1) / FP_CB;
     p.nkb = (Ce + 63) / 64;
@@ -378,7 +600,7 @@ extern "C" int lp_dw7_project_f16(const void* x, const void* w_dw, const float* 
     {
         uint64_t dims[4] = {(uint64_t)Ce, (uint64_t)W, (uint64_t)H, (uint64_t)N};
         uint64_t strides[3] = {(uint64_t)Ce * 2, (uint64_t)W * Ce * 2, (uint64_t)H * W * Ce * 2};
-        uint32_t box[4] = {(uint32_t)FP_CB, (uint32_t)FpCfg<7>::I, (uint32_t)FpCfg<7>::I, 1u};
+        uint32_t box[4] = {(uint32_t)FP_CB, (uint32_t)(wide ? FW_IX : FpCfg<7>::I), (uint32_t)(wide ? FW_IY : FpCfg<7>::I), 1u};
         int rc = make_tmap(&mx, x, 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE);
         if (rc) return rc;
         // packed projection weights: [kb][n_tile][64] (lp_pw1x1_pack with a single N chunk since Co <= 160)
@@ -396,6 +618,7 @@ extern "C" int lp_dw7_project_f16(const void* x, const void* w_dw, const float* 
         int rc = make_tmap(&md, w_dw, 2, d2, s2, b2, CU_TENSOR_MAP_SWIZZLE_NONE);
         if (rc) return rc;
     }
+    if (wide) return launch_dw_project_wide(mx, mw, md, p, (cudaStream_t)stream);
     return launch_dw_project<7, 0>(mx, mx, mw, md, p, (cudaStream_t)stream);
 }
 
