@@ -1,20 +1,18 @@
-// wgmma tensor-core contraction kernel family for LitePose on sm_90a.
+// wgmma tensor-core contraction kernel for the fusion deconv and the unfused heads of LitePose on sm_90a.
+// The 1x1 convolutions run their own kernel (pw_gemm.cu).
 //
-// One persistent, warp-specialised kernel covers the three dense contractions of the
-// network (reference lib/models/layers/layers.py:95-108, lib/models/pose_mobilenet.py:102-154):
-//   MODE_PW     1x1 conv:   out[M,N]   = act(A[M,K] W^T + b) (+res)          (InvBottleneck inv/point_conv, stem 1x1)
+// One persistent, warp-specialised kernel covers the two spatial contractions of the network
+// (reference lib/models/pose_mobilenet.py:102-154):
 //   MODE_DECONV fusion deconv level: 4 sub-pixel phases, each a K = 4*(Cr+Cw) contraction, both branches,
 //               folded-BN bias + ReLU, written interleaved into the 2x up-sampled NHWC output
 //   MODE_HEAD   head pair:  out_nchw_f32 = A1 W1^T + A2 W2^T
 //
 // Structure per CTA (384 threads, 1 CTA/SM, grid = min(#tiles, #SMs)):
-//   warp 0 lane 0 : TMA producer  (cp.async.bulk.tensor -> 128B-swizzled smem ring; MODE_PW may keep the weights of
-//                                  its N chunk resident and stream only activation tiles)
+//   warp 0 lane 0 : TMA producer  (cp.async.bulk.tensor -> 128B-swizzled smem ring)
 //   warps 4..11   : two consumer warpgroups, one per 64-row half of the 128-row tile: wgmma m64n16k16 from the ring
 //                   into fp32 register accumulators (up to 256 columns), then the epilogue straight from the
-//                   accumulator fragments (bias/act/residual -> swizzled smem staging -> TMA store, or direct stores
-//                   in the spatial modes).  The producer runs up to a ring ahead, so the next tile's loads overlap the
-//                   epilogue.
+//                   accumulator fragments (direct stores).  The producer runs up to a ring ahead, so the next tile's
+//                   loads overlap the epilogue.
 // A "step" is one 128-row x 64-channel activation tile (one TMA box; spatially shifted boxes with hardware
 // zero fill implement the deconv taps and all image borders) multiplied against 1..4 weight sub-tiles.
 #include "common.cuh"
@@ -25,19 +23,14 @@ constexpr int BM = 128;
 constexpr int BK = 64;
 constexpr int A_BYTES = BM * BK * 2;    // 16 KiB
 constexpr int B_BYTES = 256 * BK * 2;   // 32 KiB
-constexpr int STAGES = 3;        // MODE_PW (plus OUT_BYTES of output staging)
-constexpr int STAGES_NOSTAGE = 4; // MODE_DECONV / MODE_HEAD (no staging buffer)
-constexpr int MAX_STAGES = 9;      // resident-weights mode: the whole ring area minus the weights holds 16 KiB A stages
-constexpr int RING_BYTES = STAGES * (A_BYTES + B_BYTES);   // 144 KiB
-constexpr int OUT_SUB = 128 * 64 * 2;   // one 128-row x 64-column fp16 output sub-tile (128B-swizzled), 16 KiB
-constexpr int OUT_BYTES = 4 * OUT_SUB;  // staging for up to 256 output columns
+constexpr int STAGES = 4;
 constexpr int MAX_STEPS = 48;
 constexpr int GEMM_THREADS = 384;   // warpgroup 0: TMA (warp 0), warpgroups 1, 2: MMA + epilogue
 constexpr int CONS_WARPS = 8;
 constexpr int ACC_CHUNKS = 16;      // 256 accumulator columns per tile
 constexpr int MAX_BIAS = 1024;
 
-enum { MODE_PW = 0, MODE_DECONV = 1, MODE_HEAD = 2 };
+enum { MODE_DECONV = 1, MODE_HEAD = 2 };
 
 struct Step {
     int16_t kc;       // channel offset of this 64-wide K block inside its source tensor
@@ -52,45 +45,34 @@ struct Step {
 };
 
 struct GemmParams {
-    int num_tiles;     // m_tiles * n_chunks
+    int num_tiles;
     int n_chunks;
     int n_tile;        // MMA N (multiple of 16, <= 256)
     int num_steps;
     int total_bt;      // weight sub-tiles per chunk
-    int b_resident;    // MODE_PW: all K blocks of the CTA's N chunk stay in shared memory, only A tiles stream
-    int nst_a;         // MODE_PW resident mode: number of 16 KiB A stages
-    int m_tiles;
-    int M, N;          // PW: rows, real out channels.  spatial modes: N = Co
+    int N;             // Co
     int act;
-    int H, W, TH, TW, tiles_x, tiles_y;  // spatial modes
+    int H, W, TH, TW, tiles_x, tiles_y;
     const float* bias;       // packed, n_chunks*n_tile (may be null)
-    const __half* residual;  // PW only (may be null)
     void* out;
     Step steps[MAX_STEPS];
 };
 
 struct __align__(8) GemmBarriers {
-    uint64_t full[MAX_STAGES];
-    uint64_t empty[MAX_STAGES];
-    uint64_t res_full;
-    uint64_t bres_full;
+    uint64_t full[STAGES];
+    uint64_t empty[STAGES];
 };
 
-constexpr size_t GEMM_SMEM = 1024 /*align slack*/ + (size_t)STAGES * (A_BYTES + B_BYTES) + OUT_BYTES + MAX_BIAS * 4 + 256;
-
-__device__ __forceinline__ void cons_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+constexpr size_t GEMM_SMEM = 1024 /*align slack*/ + (size_t)STAGES * (A_BYTES + B_BYTES) + MAX_BIAS * 4 + 256;
 
 template <int MODE>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUtensorMap mapA1,
-               const __grid_constant__ CUtensorMap mapB, const __grid_constant__ CUtensorMap mapOut,
-               const __grid_constant__ CUtensorMap mapRes, const __grid_constant__ GemmParams p) {
+               const __grid_constant__ CUtensorMap mapB, const __grid_constant__ GemmParams p) {
     extern __shared__ __align__(1024) uint8_t smem[];
-    constexpr int NST = (MODE == MODE_PW) ? STAGES : STAGES_NOSTAGE;
     uint8_t* sA = smem;
-    uint8_t* sB = smem + NST * A_BYTES;
-    uint8_t* sOut = smem + NST * (A_BYTES + B_BYTES);      // MODE_PW: swizzled output / residual staging
-    float* sBias = reinterpret_cast<float*>(smem + STAGES * (A_BYTES + B_BYTES) + OUT_BYTES);
+    uint8_t* sB = smem + STAGES * A_BYTES;
+    float* sBias = reinterpret_cast<float*>(smem + STAGES * (A_BYTES + B_BYTES));
     GemmBarriers* bars = reinterpret_cast<GemmBarriers*>(sBias + MAX_BIAS);
 
     const int warp = threadIdx.x >> 5;
@@ -98,15 +80,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
 
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&mapA0);
-        if (MODE != MODE_PW) tma_prefetch_desc(&mapA1);
+        tma_prefetch_desc(&mapA1);
         tma_prefetch_desc(&mapB);
-        if (MODE == MODE_PW) {
-            tma_prefetch_desc(&mapOut);
-            if (p.residual) tma_prefetch_desc(&mapRes);
-        }
-        mbar_init(&bars->res_full, 1);
-        mbar_init(&bars->bres_full, 1);
-        for (int i = 0; i < MAX_STAGES; ++i) {
+        for (int i = 0; i < STAGES; ++i) {
             mbar_init(&bars->full[i], 1);
             mbar_init(&bars->empty[i], CONS_WARPS);
         }
@@ -120,66 +96,30 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
     __syncthreads();
     pdl_wait();                   // activations written by the previous kernel are complete and visible from here on
 
-    // Work distribution.  Streaming mode: item t -> (m-tile t / n_chunks, chunk t %% n_chunks), strided over the grid.
-    // Resident-weights mode (MODE_PW): the CTA keeps ONE N chunk for its whole life (its weights are loaded once),
-    // the CTAs sharing a chunk split the m-tiles round-robin.
-    const bool resident = (MODE == MODE_PW) && p.b_resident;
-    const int cpc = resident ? (int)gridDim.x / p.n_chunks : 1;           // CTAs per chunk
-    const int my_chunk = resident ? (int)blockIdx.x % p.n_chunks : 0;
-    const int t_begin = resident ? (int)blockIdx.x / p.n_chunks : (int)blockIdx.x;
-    const int t_end = resident ? p.m_tiles : p.num_tiles;
-    const int t_step = resident ? cpc : (int)gridDim.x;
-    // resident mode: weights at the start of the ring area, A stages behind them
-    const int bres_bytes = resident ? ((p.num_steps * p.n_tile * (BK * 2) + 1023) & ~1023) : 0;
-    uint8_t* sAres = smem + bres_bytes;
-    const int nst = resident ? p.nst_a : NST;
-
+    // Work distribution: item t -> (m-tile t / n_chunks, chunk t %% n_chunks), strided over the grid.
     if (warp == 0) {
         // ------------------------------------------------------------ TMA producer
         if (lane == 0) {
             uint32_t stage = 0, phase = 0;
-            if (resident) {
-                mbar_expect_tx(&bars->bres_full, (uint32_t)p.num_steps * p.n_tile * (BK * 2));
-                for (int s = 0; s < p.num_steps; ++s)
-                    tma_load_2d(smem + s * p.n_tile * (BK * 2), &mapB, &bars->bres_full, 0,
-                                (my_chunk * p.total_bt + s) * p.n_tile);
-            }
-            for (int t = t_begin; t < t_end; t += t_step) {
-                const int chunk = resident ? my_chunk : t % p.n_chunks;
-                const int mt = resident ? t : t / p.n_chunks;
-                if (resident) {
-                    for (int s = 0; s < p.num_steps; ++s) {
-                        mbar_wait_backoff(&bars->empty[stage], phase ^ 1);
-                        mbar_expect_tx(&bars->full[stage], A_BYTES);
-                        tma_load_2d(sAres + stage * A_BYTES, &mapA0, &bars->full[stage], p.steps[s].kc, mt * BM);
-                        if (++stage == (uint32_t)nst) { stage = 0; phase ^= 1; }
-                    }
-                    continue;
-                }
-                int tx = 0, ty = 0, n = 0;
-                if (MODE != MODE_PW) {
-                    tx = mt % p.tiles_x;
-                    ty = (mt / p.tiles_x) % p.tiles_y;
-                    n = mt / (p.tiles_x * p.tiles_y);
-                }
+            for (int t = blockIdx.x; t < p.num_tiles; t += gridDim.x) {
+                const int chunk = t % p.n_chunks;
+                const int mt = t / p.n_chunks;
+                const int tx = mt % p.tiles_x;
+                const int ty = (mt / p.tiles_x) % p.tiles_y;
+                const int n = mt / (p.tiles_x * p.tiles_y);
                 for (int s = 0; s < p.num_steps; ++s) {
                     const Step& st = p.steps[s];
                     mbar_wait_backoff(&bars->empty[stage], phase ^ 1);
                     const uint32_t bytes = A_BYTES + (uint32_t)st.nb * p.n_tile * (BK * 2);
                     mbar_expect_tx(&bars->full[stage], bytes);
-                    uint8_t* a_dst = sA + stage * A_BYTES;
-                    if (MODE == MODE_PW) {
-                        tma_load_2d(a_dst, &mapA0, &bars->full[stage], st.kc, mt * BM);
-                    } else {
-                        tma_load_4d(a_dst, st.map ? &mapA1 : &mapA0, &bars->full[stage], st.kc,
-                                    tx * p.TW + st.dx, ty * p.TH + st.dy, n);
-                    }
+                    tma_load_4d(sA + stage * A_BYTES, st.map ? &mapA1 : &mapA0, &bars->full[stage], st.kc,
+                                tx * p.TW + st.dx, ty * p.TH + st.dy, n);
                     uint8_t* b_dst = sB + stage * B_BYTES;
                     for (int j = 0; j < st.nb; ++j) {
                         tma_load_2d(b_dst + j * p.n_tile * (BK * 2), &mapB, &bars->full[stage], 0,
                                     (chunk * p.total_bt + st.bt0 + j) * p.n_tile);
                     }
-                    if (++stage == NST) { stage = 0; phase ^= 1; }
+                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
                 }
             }
         }
@@ -187,27 +127,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
         // ------------------------------------------------------------ consumer warpgroups: MMA + epilogue
         const int wg = (warp >> 2) - 1;            // 64-row half of the tile
         const int wq = warp & 3;
-        const bool issuer = threadIdx.x == 128;    // MODE_PW: residual loads and output stores
         const int nch = p.n_tile >> 4;
         uint32_t stage = 0, phase = 0;
-        int it = 0;
-        if (resident) mbar_wait(&bars->bres_full, 0);
-        for (int t = t_begin; t < t_end; t += t_step, ++it) {
-            const int chunk = resident ? my_chunk : t % p.n_chunks;
-            const int mt = resident ? t : t / p.n_chunks;
-            const int ncols = min(p.n_tile, p.N - chunk * p.n_tile);       // MODE_PW: valid columns of this chunk
-            const int nsub = (ncols + 63) >> 6;
-            if (MODE == MODE_PW) {
-                // the staging buffer is free once the previous tile's store has read it; the residual tile is
-                // fetched into it while this tile's MMAs run
-                if (issuer) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-                cons_sync();
-                if (p.residual && issuer) {
-                    mbar_expect_tx(&bars->res_full, nsub * OUT_SUB);
-                    for (int g = 0; g < nsub; ++g)
-                        tma_load_2d(sOut + g * OUT_SUB, &mapRes, &bars->res_full, chunk * p.n_tile + g * 64, mt * BM);
-                }
-            }
+        for (int t = blockIdx.x; t < p.num_tiles; t += gridDim.x) {
+            const int mt = t / p.n_chunks;
             float acc[ACC_CHUNKS][8];
 #pragma unroll
             for (int c = 0; c < ACC_CHUNKS; ++c)
@@ -216,8 +139,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
             for (int s = 0; s < p.num_steps; ++s) {
                 const Step& st = p.steps[s];
                 mbar_wait(&bars->full[stage], phase);
-                const uint32_t a_base = smem_u32(resident ? sAres + stage * A_BYTES : sA + stage * A_BYTES) + wg * 8192;
-                const uint32_t b_base = smem_u32(resident ? smem + s * p.n_tile * (BK * 2) : sB + stage * B_BYTES);
+                const uint32_t a_base = smem_u32(sA + stage * A_BYTES) + wg * 8192;
+                const uint32_t b_base = smem_u32(sB + stage * B_BYTES);
                 wg_fence();
                 for (int j = 0; j < st.nb; ++j) {
                     const uint32_t bj = b_base + j * p.n_tile * (BK * 2);
@@ -228,89 +151,49 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
                 wg_wait0();
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&bars->empty[stage]);
-                if (++stage == (uint32_t)nst) { stage = 0; phase ^= 1; }
+                if (++stage == STAGES) { stage = 0; phase ^= 1; }
             }
             const int rbase = wg * 64;
-            if (MODE == MODE_PW) {
-                // Output tile goes through a 128B-swizzled shared-memory staging buffer and leaves with TMA tensor
-                // stores (full 128-byte lines, rows/columns beyond M/N clipped by the tensor map); the residual tile
-                // arrives the same way.
-                if (p.residual) mbar_wait(&bars->res_full, it & 1);
+            const int tx = mt % p.tiles_x;
+            const int ty = (mt / p.tiles_x) % p.tiles_y;
+            const int n = mt / (p.tiles_x * p.tiles_y);
+            const int Co = p.N;
 #pragma unroll
-                for (int c = 0; c < ACC_CHUNKS; ++c) {
-                    if (c < nch && c * 16 < ncols) {
+            for (int i = 0; i < 4; ++i) {
+                const int row = rbase + frag_row(wq, lane, i);
+                const int ly = row / p.TW, lx = row % p.TW;
+                const int y = ty * p.TH + ly, x = tx * p.TW + lx;
+                if (y >= p.H || x >= p.W) continue;
+                if (MODE == MODE_DECONV) {
+                    __half* out = reinterpret_cast<__half*>(p.out);
 #pragma unroll
-                        for (int i = 0; i < 4; ++i) {
-                            const int row = rbase + frag_row(wq, lane, i);
-                            const int col = c * 16 + frag_col(lane, i);
-                            const int n0 = chunk * p.n_tile + col;
-                            float v0 = acc[c][2 * i] + sBias[n0], v1 = acc[c][2 * i + 1] + sBias[n0 + 1];
-                            v0 = act_apply(v0, p.act);
-                            v1 = act_apply(v1, p.act);
-                            __half2* d = reinterpret_cast<__half2*>(sOut + (col >> 6) * OUT_SUB + row * 128 +
-                                                                    ((((col & 63) >> 3) ^ (row & 7)) << 4) + (col & 7) * 2);
-                            if (p.residual) {
-                                const float2 f = __half22float2(*d);
-                                v0 += f.x;
-                                v1 += f.y;
-                            }
-                            *d = __floats2half2_rn(v0, v1);
-                        }
-                    }
-                }
-                fence_proxy_async();
-                cons_sync();
-                if (issuer) {
-                    for (int g = 0; g < nsub; ++g) {
-                        asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
-                                         reinterpret_cast<uint64_t>(&mapOut)),
-                                     "r"(smem_u32(sOut + g * OUT_SUB)), "r"(chunk * p.n_tile + g * 64), "r"(mt * BM)
-                                     : "memory");
-                    }
-                    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-                }
-            } else {
-                const int tx = mt % p.tiles_x;
-                const int ty = (mt / p.tiles_x) % p.tiles_y;
-                const int n = mt / (p.tiles_x * p.tiles_y);
-                const int Co = p.N;
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    const int row = rbase + frag_row(wq, lane, i);
-                    const int ly = row / p.TW, lx = row % p.TW;
-                    const int y = ty * p.TH + ly, x = tx * p.TW + lx;
-                    if (y >= p.H || x >= p.W) continue;
-                    if (MODE == MODE_DECONV) {
-                        __half* out = reinterpret_cast<__half*>(p.out);
-#pragma unroll
-                        for (int c = 0; c < ACC_CHUNKS; ++c) {
-                            if (c < 4 * nch) {
-                                const int ph = c / nch;                       // sub-pixel phase = accumulator index
-                                const int co = (c - ph * nch) * 16 + frag_col(lane, i);
-                                if (co < Co) {
-                                    const int a = ph >> 1, b = ph & 1;
-                                    __half* op = out + ((((long long)n * 2 * p.H + 2 * y + a) * (2 * p.W)) + 2 * x + b) * Co + co;
-                                    *reinterpret_cast<__half2*>(op) =
-                                        __floats2half2_rn(fmaxf(acc[c][2 * i] + sBias[co], 0.f),
-                                                          fmaxf(acc[c][2 * i + 1] + sBias[co + 1], 0.f));
-                                }
+                    for (int c = 0; c < ACC_CHUNKS; ++c) {
+                        if (c < 4 * nch) {
+                            const int ph = c / nch;                       // sub-pixel phase = accumulator index
+                            const int co = (c - ph * nch) * 16 + frag_col(lane, i);
+                            if (co < Co) {
+                                const int a = ph >> 1, b = ph & 1;
+                                __half* op = out + ((((long long)n * 2 * p.H + 2 * y + a) * (2 * p.W)) + 2 * x + b) * Co + co;
+                                *reinterpret_cast<__half2*>(op) =
+                                    __floats2half2_rn(fmaxf(acc[c][2 * i] + sBias[co], 0.f),
+                                                      fmaxf(acc[c][2 * i + 1] + sBias[co + 1], 0.f));
                             }
                         }
-                    } else {  // MODE_HEAD: NCHW, fp32 (act == 1) or fp16 (act == 0)
-                        const long long plane = (long long)p.H * p.W;
-                        const long long off = (long long)n * Co * plane + (long long)y * p.W + x;
-                        float* op32 = reinterpret_cast<float*>(p.out) + off;
-                        __half* op16 = reinterpret_cast<__half*>(p.out) + off;
+                    }
+                } else {  // MODE_HEAD: NCHW, fp32 (act == 1) or fp16 (act == 0)
+                    const long long plane = (long long)p.H * p.W;
+                    const long long off = (long long)n * Co * plane + (long long)y * p.W + x;
+                    float* op32 = reinterpret_cast<float*>(p.out) + off;
+                    __half* op16 = reinterpret_cast<__half*>(p.out) + off;
 #pragma unroll
-                        for (int c = 0; c < ACC_CHUNKS; ++c) {
-                            if (c < nch) {
-                                const int co = c * 16 + frag_col(lane, i);
+                    for (int c = 0; c < ACC_CHUNKS; ++c) {
+                        if (c < nch) {
+                            const int co = c * 16 + frag_col(lane, i);
 #pragma unroll
-                                for (int e = 0; e < 2; ++e) {
-                                    if (co + e < Co) {
-                                        if (p.act) op32[(long long)(co + e) * plane] = acc[c][2 * i + e];
-                                        else op16[(long long)(co + e) * plane] = __float2half_rn(acc[c][2 * i + e]);
-                                    }
+                            for (int e = 0; e < 2; ++e) {
+                                if (co + e < Co) {
+                                    if (p.act) op32[(long long)(co + e) * plane] = acc[c][2 * i + e];
+                                    else op16[(long long)(co + e) * plane] = __float2half_rn(acc[c][2 * i + e]);
                                 }
                             }
                         }
@@ -318,26 +201,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
                 }
             }
         }
-        if (MODE == MODE_PW && issuer) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
     }
 }
 
 // ------------------------------------------------------------------ host side
 static inline int round_up(int a, int b) { return (a + b - 1) / b * b; }
-
-// N <= 160 (every projection, incl. the fused depthwise+projection kernel's single-chunk layout): one chunk of
-// round_up(N,16) MMA columns.  Wider layers (the 6x expansions) are cut into 128-column chunks: a multiple of the
-// 64-column TMA store sub-tile, so stores of neighbouring chunks never overlap.
-static void pw_tiling(int N, int* n_chunks, int* n_tile) {
-    const int np = round_up(N, 16);
-    if (np <= 160) {
-        *n_chunks = 1;
-        *n_tile = np;
-        return;
-    }
-    *n_chunks = (np + 127) / 128;
-    *n_tile = 128;
-}
 
 static int set_smem_attr_once(const void* fn) {
     // cudaFuncSetAttribute is per-device state; cheap enough to set on every call
@@ -373,19 +241,13 @@ static void pick_spatial_tile(int H, int W, int* TH, int* TW) {
 }
 
 template <int MODE>
-static int launch_gemm(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const CUtensorMap& mo,
-                       const CUtensorMap& mr, const GemmParams& p, cudaStream_t stream) {
+static int launch_gemm(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const GemmParams& p,
+                       cudaStream_t stream) {
     int rc = set_smem_attr_once((const void*)gemm_tc_kernel<MODE>);
     if (rc) return rc;
-    int grid = p.num_tiles < num_sms() ? p.num_tiles : num_sms();
-    if (MODE == MODE_PW && p.b_resident) {
-        // a multiple of n_chunks CTAs, at most one per SM and no more CTAs per chunk than m-tiles
-        int cpc = num_sms() / p.n_chunks;
-        if (cpc > p.m_tiles) cpc = p.m_tiles;
-        grid = cpc * p.n_chunks;
-    }
+    const int grid = p.num_tiles < num_sms() ? p.num_tiles : num_sms();
     if (grid < 1) return LP_OK;
-    cudaError_t le = launch_pdl(gemm_tc_kernel<MODE>, dim3(grid), dim3(GEMM_THREADS), GEMM_SMEM, stream, a0, a1, b, mo, mr, p);
+    cudaError_t le = launch_pdl(gemm_tc_kernel<MODE>, dim3(grid), dim3(GEMM_THREADS), GEMM_SMEM, stream, a0, a1, b, p);
     if (le != cudaSuccess) return cuda_fail(le, "launch gemm_tc_kernel");
     LP_LAUNCH_CHECK("gemm_tc_kernel");
     return LP_OK;
@@ -394,107 +256,6 @@ static int launch_gemm(const CUtensorMap& a0, const CUtensorMap& a1, const CUten
 }  // namespace lp
 
 using namespace lp;
-
-// ------------------------------------------------------------------ pointwise 1x1
-extern "C" size_t lp_pw1x1_packed_elems(int K, int N) {
-    int nc, nt;
-    pw_tiling(N, &nc, &nt);
-    return (size_t)nc * ((K + BK - 1) / BK) * nt * BK;
-}
-extern "C" size_t lp_pw1x1_packed_bias_elems(int N) {
-    int nc, nt;
-    pw_tiling(N, &nc, &nt);
-    return (size_t)nc * nt;
-}
-extern "C" int lp_pw1x1_pack(const uint16_t* w, const float* bias, int K, int N, uint16_t* wp, float* bp) {
-    LP_CHECK_ARG(w && wp && bp && K > 0 && N > 0, "lp_pw1x1_pack: null pointer or bad shape K=%d N=%d", K, N);
-    int nc, nt;
-    pw_tiling(N, &nc, &nt);
-    const int kb = (K + BK - 1) / BK;
-    for (int c = 0; c < nc; ++c)
-        for (int s = 0; s < kb; ++s)
-            for (int r = 0; r < nt; ++r) {
-                const int n = c * nt + r;
-                uint16_t* dst = wp + (((size_t)c * kb + s) * nt + r) * BK;
-                for (int kk = 0; kk < BK; ++kk) {
-                    const int k = s * BK + kk;
-                    dst[kk] = (n < N && k < K) ? w[(size_t)n * K + k] : (uint16_t)0;
-                }
-            }
-    for (int i = 0; i < nc * nt; ++i) bp[i] = (bias && i < N) ? bias[i] : 0.f;
-    return LP_OK;
-}
-
-extern "C" int lp_pw1x1_f16(const void* a, const void* w_packed, const float* bias_packed, const void* residual,
-                            void* out, int M, int K, int N, int act, lp_stream_t stream) {
-    LP_CHECK_ARG(a && w_packed && out, "lp_pw1x1_f16: null pointer");
-    LP_CHECK_ARG(M > 0 && K >= 8 && N >= 8 && K % 8 == 0 && N % 8 == 0,
-                 "lp_pw1x1_f16: need M>0, K%%8==0, N%%8==0 (M=%d K=%d N=%d)", M, K, N);
-    LP_CHECK_ARG(act >= LP_ACT_NONE && act <= LP_ACT_RELU6, "lp_pw1x1_f16: bad act %d", act);
-    if ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(w_packed) |
-         reinterpret_cast<uintptr_t>(residual)) & 15) {
-        set_error("lp_pw1x1_f16: pointers must be 16-byte aligned");
-        return LP_ERR_ALIGN;
-    }
-    GemmParams p;
-    memset(&p, 0, sizeof(p));
-    pw_tiling(N, &p.n_chunks, &p.n_tile);
-    const int kb = (K + BK - 1) / BK;
-    LP_CHECK_ARG(kb <= MAX_STEPS && p.n_chunks * p.n_tile <= MAX_BIAS, "lp_pw1x1_f16: K=%d or N=%d too large", K, N);
-    const int m_tiles = (M + BM - 1) / BM;
-    p.num_tiles = m_tiles * p.n_chunks;
-    p.m_tiles = m_tiles;
-    p.num_steps = kb;
-    {
-        // resident-weights mode when one N chunk's weights leave room for >= 5 A stages in the ring area
-        const int bres = ((kb * p.n_tile * (BK * 2)) + 1023) & ~1023;
-        const int nst = (RING_BYTES - bres) / A_BYTES;
-        if (nst >= 5 && p.n_chunks <= num_sms()) {
-            p.b_resident = 1;
-            p.nst_a = nst < MAX_STAGES ? nst : MAX_STAGES;
-        }
-    }
-    p.total_bt = kb;
-    p.M = M;
-    p.N = N;
-    p.act = act;
-    p.bias = bias_packed;
-    p.residual = reinterpret_cast<const __half*>(residual);
-    p.out = out;
-    for (int s = 0; s < kb; ++s) {
-        Step& st = p.steps[s];
-        st.kc = (int16_t)(s * BK);
-        st.nb = 1;
-        const int kv = (K - s * BK) < BK ? (K - s * BK) : BK;
-        st.k16 = (uint8_t)((kv + 15) / 16);
-        st.acc[0] = 0;
-        st.bt0 = (uint16_t)s;
-    }
-    CUtensorMap ma, mb;
-    {
-        uint64_t dims[2] = {(uint64_t)K, (uint64_t)M};
-        uint64_t strides[1] = {(uint64_t)K * 2};
-        uint32_t box[2] = {(uint32_t)BK, (uint32_t)BM};
-        int rc = make_tmap(&ma, a, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
-        if (rc) return rc;
-        rc = make_b_map(&mb, w_packed, p.n_chunks * kb * p.n_tile, p.n_tile);
-        if (rc) return rc;
-    }
-    CUtensorMap mo, mr;
-    {
-        uint64_t dims[2] = {(uint64_t)N, (uint64_t)M};
-        uint64_t strides[1] = {(uint64_t)N * 2};
-        uint32_t box[2] = {64u, (uint32_t)BM};
-        int rc = make_tmap(&mo, out, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
-        if (rc) return rc;
-        mr = mo;
-        if (residual) {
-            rc = make_tmap(&mr, residual, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
-            if (rc) return rc;
-        }
-    }
-    return launch_gemm<MODE_PW>(ma, ma, mb, mo, mr, p, (cudaStream_t)stream);
-}
 
 // ------------------------------------------------------------------ fusion deconv
 // Two kernels share one packed-weight buffer: [tiled-kernel weights | row-kernel weights (when the channels qualify)].
@@ -618,7 +379,7 @@ extern "C" int lp_fusion_deconv_f16(const void* refined, const void* raw, const 
     if (rc) return rc;
     rc = make_b_map(&mb, w_packed, p.total_bt * p.n_tile, p.n_tile);
     if (rc) return rc;
-    return launch_gemm<MODE_DECONV>(m0, m1, mb, mb, mb, p, (cudaStream_t)stream);
+    return launch_gemm<MODE_DECONV>(m0, m1, mb, p, (cudaStream_t)stream);
 }
 
 // ------------------------------------------------------------------ heads
@@ -685,5 +446,5 @@ extern "C" int lp_head_pw_dual_f16(const void* a1, const void* a2, const void* w
     if (rc) return rc;
     rc = make_b_map(&mb, w_packed, p.total_bt * p.n_tile, p.n_tile);
     if (rc) return rc;
-    return launch_gemm<MODE_HEAD>(m0, m1, mb, mb, mb, p, (cudaStream_t)stream);
+    return launch_gemm<MODE_HEAD>(m0, m1, mb, p, (cudaStream_t)stream);
 }
