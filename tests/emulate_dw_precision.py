@@ -2,63 +2,51 @@
 
     python tests/emulate_dw_precision.py [ARCH SIZE ...]        # default: XS 128, S 128, S 256
 
-Runs the BN-folded network (oracle.model_ref.fold_bn) with fp16 storage of every activation and the stride-1 7x7 depthwise
-accumulated (a) in fp32 [mode None = what round 1 computed], (b) as fp16 row chains summed in fp32 ['rows32' = LP_DW_PREC=1],
-(c) as fp16 row chains folded by an fp16 tree ['rows' ~ the shipped grouped chains], (d) as ONE 49-tap fp16 chain ['full'],
-and prints max|out - fp32 oracle| / (2e-3 * max|ref| + 1e-4) for the two network outputs.  Measured here (round 2):
-XS/S 0.25-0.30 -> 0.28-0.35 even for (d); M 0.58 -> 0.59, L 0.44 -> 0.36: the budget is dominated by the fp16 activation
-storage, which the reference's own fp16 path shares."""
+Runs the BN-folded network (oracle.model_ref.fold_bn) with fp16 storage of every activation and every depthwise
+convolution computed by the bit-exact emulator of the kernels (tests/dw_emul.py, mirrored lanes included):
+  None  fp32 depthwise (F.conv2d)
+  0/1/2 the 7x7 and stem 3x3 depthwise at lp_set_dw_precision 0 / 1 / 2, the 5x5 heads at precision 0 -- mode 2 is the
+        shipped arithmetic (dwconv.cu default, dwpw.cu / dwblock.cu / stem_fused.cu packed chains)
+and prints max|out - fp32 oracle| / (2e-3 * max|ref| + 1e-4) for the two network outputs.  Measured (random BN-folded
+weights, synth.make_frames input):
+            None           0              1              2 (shipped)
+  XS 128    0.302 0.286    0.315 0.285    0.331 0.289    0.336 0.283
+  S 128     0.272 0.254    0.282 0.258    0.332 0.328    0.270 0.314
+  S 256     0.291 0.266    0.285 0.282    0.330 0.293    0.318 0.287
+  M 512     0.616 0.382    0.663 0.425    0.682 0.393    0.671 0.415
+The shipped arithmetic moves the ratios by at most 0.06 from an fp32 depthwise: the budget is dominated by the fp16
+activation storage, which the reference's own fp16 path shares."""
 import os, sys
 import numpy as np
 import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import torch.nn.functional as F
+import dw_emul
 from litepose_b200 import synth
 from litepose_b200.config import get_arch, get_cfg
 from litepose_b200.lib.models.pose_mobilenet import get_pose_net
 from oracle import model_ref
 
+ACTS = {None: dw_emul.ACT_NONE, "relu": dw_emul.ACT_RELU, "relu6": dw_emul.ACT_RELU6}
+
 def h(t): return t.half().float()
 
-def dw_emul(x, w, b, mode):
-    """x [N,C,H,W] fp32 holding fp16 values, w [C,1,7,7] (fp16 values), b [C] fp32. mode: 'rows' = fp16 fma chain per row, then fp16 pairwise tree over rows + bias;
-    'full' = one fp16 chain of 49; 'rows32' = fp16 row chains, fp32 sum of rows (PREC=1)"""
-    N, C, H, W = x.shape
-    xp = F.pad(x, (3, 3, 3, 3)).half()
-    wh = w.half()
-    rows = []
-    acc_full = None
-    for ky in range(7):
-        acc = None
-        for kx in range(7):
-            xs = xp[:, :, ky:ky + H, kx:kx + W]
-            ws = wh[:, 0, ky, kx].view(1, C, 1, 1)
-            prod32 = xs.float() * ws.float()
-            if mode == 'full':
-                acc_full = prod32.half() if acc_full is None else (acc_full.float() + prod32).half()   # fma: single rounding
-            else:
-                acc = prod32.half() if acc is None else (acc.float() + prod32).half()
-        rows.append(acc)
-    if mode == 'full':
-        return (acc_full.float() + b.view(1, C, 1, 1)).half().float()
-    if mode == 'rows32':
-        s = sum(r.float() for r in rows) + b.view(1, C, 1, 1)
-        return s
-    # fp16 tree: ((r0+r1)+(r2+r3)) + ((r4+r5)+(r6+bias))
-    bh = b.view(1, C, 1, 1).half().expand_as(rows[0])
-    a = (rows[0].float() + rows[1].float()).half(); b2 = (rows[2].float() + rows[3].float()).half()
-    c = (rows[4].float() + rows[5].float()).half(); d = (rows[6].float() + bh.float()).half()
-    e = (a.float() + b2.float()).half(); f = (c.float() + d.float()).half()
-    return (e.float() + f.float()).half().float()
+def dw_emul_nchw(x, w, b, stride, act, prec):
+    """x [N,C,H,W] fp32 holding fp16 values, w [C,1,k,k], b [C] -> the kernel's fp16 output (activation applied), NCHW"""
+    C, k = w.shape[0], w.shape[-1]
+    xn = x.permute(0, 2, 3, 1).contiguous().numpy().astype(np.float16)
+    wt = w.reshape(C, k * k).t().contiguous().numpy().astype(np.float16)
+    y = dw_emul.dwconv(xn, wt, b.numpy().astype(np.float32), k, stride, ACTS[act], prec)
+    return torch.from_numpy(y.astype(np.float32)).permute(0, 3, 1, 2).contiguous()
 
 def forward(fp, arch, x, mode):
     q = h
     def conv(name, x, stride=1, groups=1, act=None):
         w, b = fp[name]
-        if mode and groups > 1 and w.shape[-1] == 7 and stride == 1:
-            y = dw_emul(x, q(w), b, mode)
-        else:
-            y = F.conv2d(x, q(w), b, stride, w.shape[-1] // 2, 1, groups)
+        if mode is not None and groups > 1:
+            return dw_emul_nchw(x, q(w), b, stride, act, 0 if w.shape[-1] == 5 else mode)
+        y = F.conv2d(x, q(w), b, stride, w.shape[-1] // 2, 1, groups)
         if act == "relu6": y = F.relu6(y)
         elif act == "relu": y = F.relu(y)
         return y
@@ -102,7 +90,7 @@ for name, size in cases:
     with torch.no_grad():
         ref = model_ref.forward(sd, arch, x)
         fp = model_ref.fold_bn(sd, arch)
-        for mode in (None, 'rows32', 'rows', 'full'):
+        for mode in (None, 0, 1, 2):
             o = forward(fp, arch, x, mode)
             r = [float((a - b).abs().max() / (2e-3 * b.abs().max() + 1e-4)) for a, b in zip(o, ref)]
             print(name, size, mode, ["%.3f" % v for v in r], flush=True)
