@@ -217,6 +217,53 @@ int lp_warp_affine_normalize_u8(const uint8_t* img, int N, int H, int W, const d
                                 int out_w, int out_h, const float* mean, const float* std, void* out,
                                 int out_mode, lp_stream_t stream);
 
+/* Ragged form: N images of different sizes in ONE launch.  img is one byte buffer holding every
+ * image's [src_h][src_w][3] pixels at its src_offset; desc [N] (device) gives per image the
+ * source size, the inverted matrix (as minv above) and its output slot: dst_offset elements
+ * (of the out_mode's element type) into out, an [out_h][out_w][3] (mode 0) or [3][out_h][out_w]
+ * block.  max_out_w / max_out_h bound every out_w / out_h (they size the grid).  Per image the
+ * result is bit-identical to lp_warp_affine_normalize_u8 on that image alone (same device code). */
+typedef struct {
+    int64_t src_offset;      /* bytes */
+    int32_t src_h, src_w;
+    double minv[6];
+    int64_t dst_offset;      /* elements */
+    int32_t out_h, out_w;
+} lp_warp_desc_t;
+int lp_warp_affine_normalize_ragged_u8(const uint8_t* img, int N, const lp_warp_desc_t* desc,
+                                       int max_out_w, int max_out_h, const float* mean,
+                                       const float* std, void* out, int out_mode, lp_stream_t stream);
+
+/* ---- ragged parser: the G1-G6 chain on a det/tag arena of differently sized maps ----------
+ * det holds image n's [J,h,w] block at desc[n].det_offset, tag its [J,h,w,T] block at
+ * desc[n].tag_offset (elements).  hw_host [N][2] (HOST memory) lists the same (h, w) pairs as
+ * desc (device); it sizes the grids and the workspaces.  Outputs keep the uniform layouts
+ * (val_k [N,J,K], ans [N,pcap,J,3+T], ...) and per image equal, bit for bit, the uniform entry
+ * points run on that image alone: they share the device code, a uniform call derives the
+ * offsets from N, H, W, a ragged call reads them from desc.  Tag matching and adjust/refine
+ * need the workspaces of lp_tag_match_workspace_bytes / lp_adjust_refine_workspace_bytes. */
+typedef struct {
+    int32_t h, w;
+    int64_t det_offset;      /* elements */
+    int64_t tag_offset;      /* elements */
+} lp_map_desc_t;
+size_t lp_nms_topk_ragged_workspace_bytes(int N, const int32_t* hw_host, int J, int K);
+int lp_nms_topk_ragged_f32(const float* det, const float* tag, int N, const int32_t* hw_host,
+                           const lp_map_desc_t* desc, int J, int T, int nms_kernel, int K,
+                           double min_value, float* val_k, int32_t* ind_k, float* tag_k,
+                           void* workspace, size_t workspace_bytes, lp_stream_t stream);
+int lp_tag_match_ragged_f32(const float* val_k, const int32_t* ind_k, const float* tag_k, int N,
+                            int J, int K, int T, const lp_map_desc_t* desc,
+                            const int32_t* joint_order, double det_threshold,
+                            double tag_threshold, int use_detection_val, int ignore_too_much,
+                            int max_num_people, int pcap, float* ans, int32_t* num_people,
+                            void* workspace, size_t workspace_bytes, lp_stream_t stream);
+int lp_adjust_refine_ragged_f32(const float* det, const float* tag, int N, const int32_t* hw_host,
+                                const lp_map_desc_t* desc, int J, int T, int pcap, float* ans,
+                                const int32_t* num_people, float* scores, int do_adjust,
+                                int do_refine, void* workspace, size_t workspace_bytes,
+                                lp_stream_t stream);
+
 /* ---- final predictions ("next" row 3, post-processing side) ----------------------
  * get_final_preds (lib/utils/transforms.py:195-202): in place, x and y of every keypoint of
  * the first min(num_people[n], pcap) persons of image n go through trans[n] (row-major 2x3

@@ -71,6 +71,12 @@ SIGNATURES = {
     "lp_pack_payload_f32": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
     "lp_plant_crowd_f32": (_i, [_vp, _vp, _vp, _c.c_int64, _vp, _vp, _vp, _c.c_int64, _vp]),
     "lp_warp_affine_normalize_u8": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _i, _vp]),
+    "lp_warp_affine_normalize_ragged_u8": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _vp, _i, _vp]),
+    "lp_nms_topk_ragged_workspace_bytes": (_sz, [_i, _vp, _i, _i]),
+    "lp_nms_topk_ragged_f32": (_i, [_vp, _vp, _i, _vp, _vp, _i, _i, _i, _i, _d, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "lp_tag_match_ragged_f32": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _d, _d, _i, _i, _i, _i, _vp, _vp, _vp, _sz,
+                                     _vp]),
+    "lp_adjust_refine_ragged_f32": (_i, [_vp, _vp, _i, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _i, _i, _vp, _sz, _vp]),
     "lp_transform_preds_f32": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "lp_find_peaks_f32": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _f, _i, _vp, _vp, _vp, _vp, _vp]),
     "lp_assign_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _f, _vp, _vp, _vp, _vp]),

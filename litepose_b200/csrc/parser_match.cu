@@ -160,6 +160,7 @@ __device__ float np_pairwise_sum_f32(const float* a, int n, int stride) {
 struct MatchArgs {
     const float* val_k; const int32_t* ind_k; const float* tag_k;
     int N, J, K, T, W;
+    const lp_map_desc_t* desc;                   // ragged call: per-image map width desc[n].w (else W)
     const int32_t* joint_order;
     double det_thr, tag_thr;
     int use_det_val, ignore_too_much, max_people, pcap;
@@ -183,6 +184,7 @@ tag_match_kernel(const MatchArgs a) {
     const int n = blockIdx.x;
     const int lane = threadIdx.x;
     const int J = a.J, K = a.K, T = a.T, D = 3 + a.T;
+    const int W = a.desc ? a.desc[n].w : a.W;
     float* ans = a.ans + (size_t)n * a.pcap * J * D;
     float* pkey = a.pkey + (size_t)n * a.pcap;
     int32_t* ptagn = a.ptagn + (size_t)n * a.pcap;
@@ -232,8 +234,8 @@ tag_match_kernel(const MatchArgs a) {
         if (ok) {
             const int r = __popc(mask & ((1u << lane) - 1u));
             const int ind = a.ind_k[base + lane];
-            S.cx[r] = ind % a.W;
-            S.cy[r] = ind / a.W;
+            S.cx[r] = ind % W;
+            S.cy[r] = ind / W;
             S.cv[r] = v;
             for (int t = 0; t < T; ++t) S.ct[r][t] = a.tag_k[(base + lane) * T + t];
         }
@@ -456,6 +458,7 @@ tag_match_wide_kernel(const MatchArgs a) {
     const int n = blockIdx.x;
     const int lane = threadIdx.x;
     const int J = a.J, K = a.K, T = a.T, D = 3 + a.T;
+    const int W = a.desc ? a.desc[n].w : a.W;
     float* ans = a.ans + (size_t)n * a.pcap * J * D;
     float* pkey = a.pkey + (size_t)n * a.pcap;
     int32_t* ptagn = a.ptagn + (size_t)n * a.pcap;
@@ -509,8 +512,8 @@ tag_match_wide_kernel(const MatchArgs a) {
             if (ok[s]) {
                 const int r = __popcll(mask & ((1ull << k) - 1ull));
                 const int ind = a.ind_k[base + k];
-                S.cx[r] = ind % a.W;
-                S.cy[r] = ind / a.W;
+                S.cx[r] = ind % W;
+                S.cy[r] = ind / W;
                 S.cv[r] = v[s];
                 for (int t = 0; t < T; ++t) S.ct[r][t] = a.tag_k[(base + k) * T + t];
             }
@@ -600,25 +603,27 @@ extern "C" size_t lp_tag_match_workspace_bytes(int N, int J, int K, int T, int p
     return (size_t)N * pcap * (sizeof(float) + sizeof(int32_t) + (size_t)J * T * sizeof(float));
 }
 
-extern "C" int lp_tag_match_f32(const float* val_k, const int32_t* ind_k, const float* tag_k, int N, int J, int K, int T,
-                                int W, const int32_t* joint_order, double det_threshold, double tag_threshold,
-                                int use_detection_val, int ignore_too_much, int max_num_people, int pcap, float* ans,
-                                int32_t* num_people, void* workspace, size_t workspace_bytes, lp_stream_t stream) {
-    LP_CHECK_ARG(val_k && ind_k && tag_k && joint_order && ans && num_people && workspace, "lp_tag_match_f32: null pointer");
-    LP_CHECK_ARG(N > 0 && J > 0 && J <= 32 && K > 0 && K <= MW && T > 0 && T < 8 && W > 0,
-                 "lp_tag_match_f32: bad shape N=%d J=%d K=%d T=%d (J<=32, K<=64, T<8)", N, J, K, T);
-    LP_CHECK_ARG(max_num_people > 0 && max_num_people <= MW, "lp_tag_match_f32: max_num_people=%d out of range (1..64)",
+// Both entry points: W > 0 (uniform) or desc != nullptr (ragged).
+static int tag_match_launch(const float* val_k, const int32_t* ind_k, const float* tag_k, int N, int J, int K, int T,
+                            int W, const lp_map_desc_t* desc, const int32_t* joint_order, double det_threshold,
+                            double tag_threshold, int use_detection_val, int ignore_too_much, int max_num_people, int pcap,
+                            float* ans, int32_t* num_people, void* workspace, size_t workspace_bytes, lp_stream_t stream,
+                            const char* name) {
+    LP_CHECK_ARG(val_k && ind_k && tag_k && joint_order && ans && num_people && workspace, "%s: null pointer", name);
+    LP_CHECK_ARG(N > 0 && J > 0 && J <= 32 && K > 0 && K <= MW && T > 0 && T < 8 && (W > 0 || desc),
+                 "%s: bad shape N=%d J=%d K=%d T=%d (J<=32, K<=64, T<8)", name, N, J, K, T);
+    LP_CHECK_ARG(max_num_people > 0 && max_num_people <= MW, "%s: max_num_people=%d out of range (1..64)", name,
                  max_num_people);
-    LP_CHECK_ARG(pcap >= max_num_people, "lp_tag_match_f32: pcap=%d must be >= max_num_people=%d", pcap, max_num_people);
-    LP_CHECK_ARG(det_threshold >= 0.0, "lp_tag_match_f32: detection threshold must be >= 0");
+    LP_CHECK_ARG(pcap >= max_num_people, "%s: pcap=%d must be >= max_num_people=%d", name, pcap, max_num_people);
+    LP_CHECK_ARG(det_threshold >= 0.0, "%s: detection threshold must be >= 0", name);
     const size_t need = lp_tag_match_workspace_bytes(N, J, K, T, pcap);
     if (workspace_bytes < need) {
-        set_error("lp_tag_match_f32: workspace %zu < required %zu bytes", workspace_bytes, need);
+        set_error("%s: workspace %zu < required %zu bytes", name, workspace_bytes, need);
         return LP_ERR_CAPACITY;
     }
     MatchArgs a;
     a.val_k = val_k; a.ind_k = ind_k; a.tag_k = tag_k;
-    a.N = N; a.J = J; a.K = K; a.T = T; a.W = W;
+    a.N = N; a.J = J; a.K = K; a.T = T; a.W = W; a.desc = desc;
     a.joint_order = joint_order;
     a.det_thr = det_threshold; a.tag_thr = tag_threshold;
     a.use_det_val = use_detection_val; a.ignore_too_much = ignore_too_much;
@@ -642,4 +647,25 @@ extern "C" int lp_tag_match_f32(const float* val_k, const int32_t* ind_k, const 
     tag_match_kernel<<<N, 32, 0, (cudaStream_t)stream>>>(a);
     LP_LAUNCH_CHECK("tag_match_kernel");
     return LP_OK;
+}
+
+extern "C" int lp_tag_match_f32(const float* val_k, const int32_t* ind_k, const float* tag_k, int N, int J, int K, int T,
+                                int W, const int32_t* joint_order, double det_threshold, double tag_threshold,
+                                int use_detection_val, int ignore_too_much, int max_num_people, int pcap, float* ans,
+                                int32_t* num_people, void* workspace, size_t workspace_bytes, lp_stream_t stream) {
+    LP_CHECK_ARG(W > 0, "lp_tag_match_f32: bad shape W=%d", W);
+    return tag_match_launch(val_k, ind_k, tag_k, N, J, K, T, W, nullptr, joint_order, det_threshold, tag_threshold,
+                            use_detection_val, ignore_too_much, max_num_people, pcap, ans, num_people, workspace,
+                            workspace_bytes, stream, "lp_tag_match_f32");
+}
+
+extern "C" int lp_tag_match_ragged_f32(const float* val_k, const int32_t* ind_k, const float* tag_k, int N, int J, int K,
+                                       int T, const lp_map_desc_t* desc, const int32_t* joint_order, double det_threshold,
+                                       double tag_threshold, int use_detection_val, int ignore_too_much,
+                                       int max_num_people, int pcap, float* ans, int32_t* num_people, void* workspace,
+                                       size_t workspace_bytes, lp_stream_t stream) {
+    LP_CHECK_ARG(desc, "lp_tag_match_ragged_f32: null pointer");
+    return tag_match_launch(val_k, ind_k, tag_k, N, J, K, T, 0, desc, joint_order, det_threshold, tag_threshold,
+                            use_detection_val, ignore_too_much, max_num_people, pcap, ans, num_people, workspace,
+                            workspace_bytes, stream, "lp_tag_match_ragged_f32");
 }

@@ -25,6 +25,29 @@ struct RefineWs {
     unsigned long long* best;     // [N][pcap][J]
 };
 
+// Maps of image n.  Uniform call (desc == nullptr): [N,J,H,W] det and [N,J,H,W,T] tag.  Ragged call: desc[n] gives the
+// size and the offsets of the image's blocks in the det / tag arena.
+struct ImageMaps {
+    int H, W;
+    size_t det_off, tag_off;
+};
+
+__device__ __forceinline__ ImageMaps image_maps(const lp_map_desc_t* desc, int n, int J, int H, int W, int T) {
+    ImageMaps m;
+    if (desc == nullptr) {
+        m.H = H;
+        m.W = W;
+        m.det_off = (size_t)n * J * H * W;
+        m.tag_off = (size_t)n * J * H * W * T;
+    } else {
+        m.H = desc[n].h;
+        m.W = desc[n].w;
+        m.det_off = (size_t)desc[n].det_offset;
+        m.tag_off = (size_t)desc[n].tag_offset;
+    }
+    return m;
+}
+
 __device__ __forceinline__ float np_mean_pairwise(const float* a, int n, int stride) {
     // numpy add.reduce (pairwise, 8 accumulators) / n for n < 128
     float res;
@@ -48,15 +71,18 @@ __device__ __forceinline__ float np_mean_pairwise(const float* a, int n, int str
 
 // one CTA per image
 __global__ void __launch_bounds__(128)
-adjust_scores_kernel(const float* __restrict__ det, const float* __restrict__ tag, int J, int H, int W, int T, int pcap,
-                     float* __restrict__ ans_all, const int32_t* __restrict__ num_people, float* __restrict__ scores_all,
-                     int do_adjust, int do_refine, RefineWs ws) {
+adjust_scores_kernel(const float* __restrict__ det, const float* __restrict__ tag, const lp_map_desc_t* __restrict__ desc,
+                     int J, int H_u, int W_u, int T, int pcap, float* __restrict__ ans_all,
+                     const int32_t* __restrict__ num_people, float* __restrict__ scores_all, int do_adjust, int do_refine,
+                     RefineWs ws) {
     const int n = blockIdx.x;
     const int D = 3 + T;
     const int P = min(num_people[n], pcap);
+    const ImageMaps im = image_maps(desc, n, J, H_u, W_u, T);
+    const int H = im.H, W = im.W;
     float* ans = ans_all + (size_t)n * pcap * J * D;
-    const float* detn = det + (size_t)n * J * H * W;
-    const float* tagn = tag + (size_t)n * J * H * W * T;
+    const float* detn = det + im.det_off;
+    const float* tagn = tag + im.tag_off;
 
     if (do_refine) {
         for (int i = threadIdx.x; i < J; i += blockDim.x) ws.miss_cnt[(size_t)n * J + i] = 0;
@@ -137,17 +163,21 @@ __device__ __forceinline__ unsigned long long warp_max_u64(unsigned long long v)
 
 template <int T>
 __global__ void __launch_bounds__(RF_THREADS)
-refine_argmax_kernel(const float* __restrict__ det, const float* __restrict__ tag, int J, int HW, int pcap, RefineWs ws) {
+refine_argmax_kernel(const float* __restrict__ det, const float* __restrict__ tag, const lp_map_desc_t* __restrict__ desc,
+                     int J, int H_u, int W_u, int pcap, RefineWs ws) {
     const int n = blockIdx.z, j = blockIdx.y;
+    const ImageMaps im = image_maps(desc, n, J, H_u, W_u, T);
+    const int HW = im.H * im.W;
+    const int pix0 = blockIdx.x * RF_CHUNK;
+    if (pix0 >= HW) return;                        // ragged: the grid covers the largest map
     const int cnt = ws.miss_cnt[(size_t)n * J + j];
     if (cnt == 0) return;
     __shared__ unsigned long long s_best[RF_PB];
     __shared__ float s_prev[RF_PB][RF_TMAX];
     __shared__ int s_pid[RF_PB];
     const size_t plane = (size_t)n * J + j;
-    const float* dp = det + plane * HW;
-    const float* tp = tag + plane * HW * T;
-    const int pix0 = blockIdx.x * RF_CHUNK;
+    const float* dp = det + im.det_off + (size_t)j * HW;
+    const float* tp = tag + im.tag_off + (size_t)j * HW * T;
     float d[RF_PIX], tg[RF_PIX][T];
 #pragma unroll
     for (int k = 0; k < RF_PIX; ++k) {
@@ -204,12 +234,14 @@ refine_argmax_kernel(const float* __restrict__ det, const float* __restrict__ ta
 }
 
 __global__ void __launch_bounds__(128)
-refine_finalize_kernel(const float* __restrict__ det, int J, int H, int W, int T, int pcap, float* __restrict__ ans_all,
-                       RefineWs ws) {
+refine_finalize_kernel(const float* __restrict__ det, const lp_map_desc_t* __restrict__ desc, int J, int H_u, int W_u,
+                       int T, int pcap, float* __restrict__ ans_all, RefineWs ws) {
     const int n = blockIdx.y, j = blockIdx.x;
     const int cnt = ws.miss_cnt[(size_t)n * J + j];
     const int D = 3 + T;
-    const float* tmp = det + ((size_t)n * J + j) * H * W;
+    const ImageMaps im = image_maps(desc, n, J, H_u, W_u, T);
+    const int H = im.H, W = im.W;
+    const float* tmp = det + im.det_off + (size_t)j * H * W;
     for (int q = threadIdx.x; q < cnt; q += blockDim.x) {
         const int p = ws.miss_list[((size_t)n * J + j) * pcap + q];
         const unsigned long long key = ws.best[((size_t)n * pcap + p) * J + j];
@@ -245,20 +277,27 @@ extern "C" size_t lp_adjust_refine_workspace_bytes(int N, int J, int pcap) {
     return b;
 }
 
-extern "C" int lp_adjust_refine_f32(const float* det, const float* tag, int N, int J, int H, int W, int T, int pcap,
-                                    float* ans, const int32_t* num_people, float* scores, int do_adjust, int do_refine,
-                                    void* workspace, size_t workspace_bytes, lp_stream_t stream) {
-    LP_CHECK_ARG(det && tag && ans && num_people && scores && workspace, "lp_adjust_refine_f32: null pointer");
-    LP_CHECK_ARG(N > 0 && N <= 65535 && J > 0 && J <= 65535 && H > 0 && W > 0 && pcap > 0 && (long long)H * W < (1ll << 31),
-                 "lp_adjust_refine_f32: bad shape N=%d J=%d H=%d W=%d pcap=%d", N, J, H, W, pcap);
-    LP_CHECK_ARG(T >= 1 && T <= RF_TMAX, "lp_adjust_refine_f32: T=%d unsupported (1..%d)", T, RF_TMAX);
+// Both entry points: uniform (hw_host == nullptr, every map H x W) or ragged (per-image sizes, device desc).
+static int adjust_refine_launch(const float* det, const float* tag, int N, const int32_t* hw_host, const lp_map_desc_t* desc,
+                                int J, int H, int W, int T, int pcap, float* ans, const int32_t* num_people, float* scores,
+                                int do_adjust, int do_refine, void* workspace, size_t workspace_bytes, lp_stream_t stream,
+                                const char* name) {
+    LP_CHECK_ARG(det && tag && ans && num_people && scores && workspace, "%s: null pointer", name);
+    LP_CHECK_ARG(N > 0 && N <= 65535 && J > 0 && J <= 65535 && pcap > 0, "%s: bad shape N=%d J=%d pcap=%d", name, N, J, pcap);
+    LP_CHECK_ARG(T >= 1 && T <= RF_TMAX, "%s: T=%d unsupported (1..%d)", name, T, RF_TMAX);
+    long long max_hw = 0;
+    for (int n = 0; n < (hw_host ? N : 1); ++n) {
+        const int h = hw_host ? hw_host[2 * n] : H, w = hw_host ? hw_host[2 * n + 1] : W;
+        LP_CHECK_ARG(h > 0 && w > 0 && (long long)h * w < (1ll << 31), "%s: bad map size %dx%d (image %d)", name, h, w, n);
+        max_hw = (long long)h * w > max_hw ? (long long)h * w : max_hw;
+    }
     const size_t need = lp_adjust_refine_workspace_bytes(N, J, pcap);
     if (workspace_bytes < need) {
-        set_error("lp_adjust_refine_f32: workspace %zu < required %zu bytes", workspace_bytes, need);
+        set_error("%s: workspace %zu < required %zu bytes", name, workspace_bytes, need);
         return LP_ERR_CAPACITY;
     }
     if (reinterpret_cast<uintptr_t>(workspace) & 255) {
-        set_error("lp_adjust_refine_f32: workspace must be 256-byte aligned");
+        set_error("%s: workspace must be 256-byte aligned", name);
         return LP_ERR_ALIGN;
     }
     RefineWs ws;
@@ -271,23 +310,40 @@ extern "C" int lp_adjust_refine_f32(const float* det, const float* tag, int N, i
     b += align_up((size_t)N * J * pcap * sizeof(int32_t), 256);
     ws.best = reinterpret_cast<unsigned long long*>(b);
     cudaStream_t s = (cudaStream_t)stream;
-    adjust_scores_kernel<<<N, 128, 0, s>>>(det, tag, J, H, W, T, pcap, ans, num_people, scores, do_adjust, do_refine, ws);
+    adjust_scores_kernel<<<N, 128, 0, s>>>(det, tag, desc, J, H, W, T, pcap, ans, num_people, scores, do_adjust, do_refine,
+                                           ws);
     LP_LAUNCH_CHECK("adjust_scores_kernel");
     if (do_refine) {
-        const int HW = H * W;
-        dim3 grid((HW + RF_CHUNK - 1) / RF_CHUNK, J, N);
+        dim3 grid((unsigned)((max_hw + RF_CHUNK - 1) / RF_CHUNK), J, N);
         switch (T) {
-            case 1: refine_argmax_kernel<1><<<grid, RF_THREADS, 0, s>>>(det, tag, J, HW, pcap, ws); break;
-            case 2: refine_argmax_kernel<2><<<grid, RF_THREADS, 0, s>>>(det, tag, J, HW, pcap, ws); break;
-            case 3: refine_argmax_kernel<3><<<grid, RF_THREADS, 0, s>>>(det, tag, J, HW, pcap, ws); break;
-            default: refine_argmax_kernel<4><<<grid, RF_THREADS, 0, s>>>(det, tag, J, HW, pcap, ws); break;
+            case 1: refine_argmax_kernel<1><<<grid, RF_THREADS, 0, s>>>(det, tag, desc, J, H, W, pcap, ws); break;
+            case 2: refine_argmax_kernel<2><<<grid, RF_THREADS, 0, s>>>(det, tag, desc, J, H, W, pcap, ws); break;
+            case 3: refine_argmax_kernel<3><<<grid, RF_THREADS, 0, s>>>(det, tag, desc, J, H, W, pcap, ws); break;
+            default: refine_argmax_kernel<4><<<grid, RF_THREADS, 0, s>>>(det, tag, desc, J, H, W, pcap, ws); break;
         }
         LP_LAUNCH_CHECK("refine_argmax_kernel");
         dim3 g2(J, N);
-        refine_finalize_kernel<<<g2, 128, 0, s>>>(det, J, H, W, T, pcap, ans, ws);
+        refine_finalize_kernel<<<g2, 128, 0, s>>>(det, desc, J, H, W, T, pcap, ans, ws);
         LP_LAUNCH_CHECK("refine_finalize_kernel");
     }
     return LP_OK;
+}
+
+extern "C" int lp_adjust_refine_f32(const float* det, const float* tag, int N, int J, int H, int W, int T, int pcap,
+                                    float* ans, const int32_t* num_people, float* scores, int do_adjust, int do_refine,
+                                    void* workspace, size_t workspace_bytes, lp_stream_t stream) {
+    LP_CHECK_ARG(H > 0 && W > 0, "lp_adjust_refine_f32: bad shape N=%d J=%d H=%d W=%d pcap=%d", N, J, H, W, pcap);
+    return adjust_refine_launch(det, tag, N, nullptr, nullptr, J, H, W, T, pcap, ans, num_people, scores, do_adjust,
+                                do_refine, workspace, workspace_bytes, stream, "lp_adjust_refine_f32");
+}
+
+extern "C" int lp_adjust_refine_ragged_f32(const float* det, const float* tag, int N, const int32_t* hw_host,
+                                           const lp_map_desc_t* desc, int J, int T, int pcap, float* ans,
+                                           const int32_t* num_people, float* scores, int do_adjust, int do_refine,
+                                           void* workspace, size_t workspace_bytes, lp_stream_t stream) {
+    LP_CHECK_ARG(hw_host && desc, "lp_adjust_refine_ragged_f32: null pointer");
+    return adjust_refine_launch(det, tag, N, hw_host, desc, J, 0, 0, T, pcap, ans, num_people, scores, do_adjust,
+                                do_refine, workspace, workspace_bytes, stream, "lp_adjust_refine_ragged_f32");
 }
 
 // ---------------------------------------------------------------------------------------------- final predictions

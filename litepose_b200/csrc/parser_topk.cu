@@ -26,7 +26,7 @@ __device__ __forceinline__ unsigned long long shfl_max_u64(unsigned long long v)
     return v;
 }
 
-static inline int strip_rows(int W) {
+__host__ __device__ inline int strip_rows(int W) {
     // keep both shared planes (rows + halo) under ~96 KB
     int sr = 16;
     while (sr > 2 && (size_t)(sr + 8) * W * 8 > 96 * 1024) sr >>= 1;
@@ -34,6 +34,11 @@ static inline int strip_rows(int W) {
 }
 
 constexpr int TK_SPB = 4;        // strips walked sequentially by one CTA (a "band")
+
+__host__ __device__ inline int plane_bands(int H, int W) {
+    const int sr = strip_rows(W);
+    return ((H + sr - 1) / sr + TK_SPB - 1) / TK_SPB;
+}
 
 // Sorted insert of `key` into the descending list s_top[0..ntop) (capacity K <= 64) by one warp.
 __device__ __forceinline__ int topk_insert(unsigned long long* s_top, int ntop, int K, unsigned long long key, int lane) {
@@ -57,7 +62,40 @@ __device__ __forceinline__ int topk_insert(unsigned long long* s_top, int ntop, 
 
 constexpr int TK_WARPS = TK_THREADS / 32;
 
-// partial: [N*J][bands * TK_WARPS][K] keys (sorted, 0 = empty); plane_thr: [N*J] running lower bound of the plane's
+// Geometry of one (image, joint) plane.  Uniform call (desc == nullptr): every plane is H x W, planes are adjacent, the
+// per-warp candidate lists of plane p start at p * nbands * TK_WARPS * K.  Ragged call: image n = plane / J has its own
+// size and det / tag offsets (desc[n]); its lists follow those of images 0..n-1 (prefix sum over the images).
+struct PlaneGeom {
+    int H, W, SR, nbands;
+    size_t det_off, tag_off, list_off;
+};
+
+__device__ __forceinline__ PlaneGeom plane_geom(const lp_map_desc_t* desc, int plane, int J, int H, int W, int T, int K) {
+    PlaneGeom g;
+    if (desc == nullptr) {
+        g.H = H;
+        g.W = W;
+        g.SR = strip_rows(W);
+        g.nbands = plane_bands(H, W);
+        g.det_off = (size_t)plane * H * W;
+        g.tag_off = (size_t)plane * H * W * T;
+        g.list_off = (size_t)plane * g.nbands * TK_WARPS * K;
+        return g;
+    }
+    const int n = plane / J, j = plane - n * J;
+    size_t lists = 0;
+    for (int i = 0; i < n; ++i) lists += (size_t)J * plane_bands(desc[i].h, desc[i].w) * TK_WARPS * K;
+    g.H = desc[n].h;
+    g.W = desc[n].w;
+    g.SR = strip_rows(g.W);
+    g.nbands = plane_bands(g.H, g.W);
+    g.det_off = (size_t)desc[n].det_offset + (size_t)j * g.H * g.W;
+    g.tag_off = (size_t)desc[n].tag_offset + (size_t)j * g.H * g.W * T;
+    g.list_off = lists + (size_t)j * g.nbands * TK_WARPS * K;
+    return g;
+}
+
+// partial: per plane [bands * TK_WARPS][K] keys (PlaneGeom::list_off) (sorted, 0 = empty); plane_thr: [N*J] running lower bound of the plane's
 // K-th key (zero-initialised by the caller).  One CTA walks TK_SPB strips of SR rows of one plane; inside a strip every
 // warp owns the rows r == warp (mod 8) and keeps its OWN sorted top-K list (no block barriers, no serial merge).  A pixel
 // can only matter if its key reaches the best known K-th key -- the maximum over all warps of the CTA (shared memory)
@@ -65,15 +103,19 @@ constexpr int TK_WARPS = TK_THREADS / 32;
 // K-th key -- so the k x k window maximum (the NMS test) is evaluated for a vanishing fraction of pixels and the
 // kernel streams at memory speed.  The per-warp lists are merged by topk_merge_kernel.
 __global__ void __launch_bounds__(TK_THREADS)
-nms_topk_strip_kernel(const float* __restrict__ det, int H, int W, int R /*window radius*/, int SR, int K, float floor_v,
-                      unsigned long long* __restrict__ partial, unsigned long long* __restrict__ plane_thr) {
+nms_topk_strip_kernel(const float* __restrict__ det, const lp_map_desc_t* __restrict__ desc, int J, int H_u, int W_u,
+                      int R /*window radius*/, int K, float floor_v, unsigned long long* __restrict__ partial,
+                      unsigned long long* __restrict__ plane_thr) {
     extern __shared__ __align__(16) float sm[];
     const int plane = blockIdx.y;
-    const int band = blockIdx.x, nbands = gridDim.x;
+    const PlaneGeom geo = plane_geom(desc, plane, J, H_u, W_u, 1, K);
+    const int band = blockIdx.x;
+    if (band >= geo.nbands) return;                // ragged: the grid covers the image with the most bands
+    const int H = geo.H, W = geo.W, SR = geo.SR;
     float* s_val = sm;                             // [SR+2R][W] raw values (out-of-image rows hold -inf)
     __shared__ unsigned long long s_top[TK_WARPS][TK_MAXK];
     __shared__ unsigned long long s_thr;           // CTA-wide lower bound of the K-th key
-    const float* p = det + (size_t)plane * H * W;
+    const float* p = det + geo.det_off;
     const float NEG_INF = __int_as_float(0xff800000);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     for (int i = lane; i < TK_MAXK; i += 32) s_top[warp][i] = 0ull;
@@ -197,17 +239,21 @@ nms_topk_strip_kernel(const float* __restrict__ det, int H, int W, int R /*windo
         if (lane == 0 && thr) atomicMax(plane_thr + plane, thr);
     }
     __syncwarp();
-    unsigned long long* out = partial + (((size_t)plane * nbands + band) * TK_WARPS + warp) * K;
+    unsigned long long* out = partial + geo.list_off + ((size_t)band * TK_WARPS + warp) * K;
     for (int k = lane; k < K; k += 32) out[k] = k < ntop ? mytop[k] : 0ull;
 }
 
 // one warp per plane
 __global__ void __launch_bounds__(32)
-topk_merge_kernel(const unsigned long long* __restrict__ partial, const float* __restrict__ tag, int HW, int T,
-                  int nstrips, int K, float* __restrict__ val_k, int32_t* __restrict__ ind_k, float* __restrict__ tag_k) {
+topk_merge_kernel(const unsigned long long* __restrict__ partial, const float* __restrict__ tag,
+                  const lp_map_desc_t* __restrict__ desc, int J, int H_u, int W_u, int T, int K, float* __restrict__ val_k,
+                  int32_t* __restrict__ ind_k, float* __restrict__ tag_k) {
     const int plane = blockIdx.x;
     const int lane = threadIdx.x;
-    const unsigned long long* pl = partial + (size_t)plane * nstrips * K;
+    const PlaneGeom geo = plane_geom(desc, plane, J, H_u, W_u, T, K);
+    const int nstrips = geo.nbands * TK_WARPS;
+    const unsigned long long* pl = partial + geo.list_off;
+    const float* tg = tag + geo.tag_off;
     // each lane owns strips lane, lane+32, ...; head[] = cursor into each sorted strip list
     constexpr int MAXS = 8;   // up to 256 strips
     int head[MAXS];
@@ -240,7 +286,7 @@ topk_merge_kernel(const unsigned long long* __restrict__ partial, const float* _
             val_k[(size_t)plane * K + k] = v;
             ind_k[(size_t)plane * K + k] = idx;
             for (int t = 0; t < T; ++t)
-                tag_k[((size_t)plane * K + k) * T + t] = __ldg(tag + ((size_t)plane * HW + idx) * T + t);
+                tag_k[((size_t)plane * K + k) * T + t] = __ldg(tg + (size_t)idx * T + t);
         }
     }
 }
@@ -249,54 +295,97 @@ topk_merge_kernel(const unsigned long long* __restrict__ partial, const float* _
 
 using namespace lp;
 
-extern "C" size_t lp_nms_topk_workspace_bytes(int N, int J, int H, int W, int K) {
-    if (N <= 0 || J <= 0 || H <= 0 || W <= 0 || K <= 0) return 0;
-    const int sr = strip_rows(W);
-    const int nstrips = ((H + sr - 1) / sr + TK_SPB - 1) / TK_SPB;   // bands of TK_SPB strips
-    // per-warp candidate lists + one running threshold per plane
-    return (size_t)N * J * nstrips * TK_WARPS * K * sizeof(unsigned long long) + (size_t)N * J * sizeof(unsigned long long);
+static size_t topk_list_bytes(int J, int H, int W, int K) {
+    return (size_t)J * plane_bands(H, W) * TK_WARPS * K * sizeof(unsigned long long);
 }
 
-extern "C" int lp_nms_topk_f32(const float* det, const float* tag, int N, int J, int H, int W, int T, int nms_kernel,
-                               int K, double min_value, float* val_k, int32_t* ind_k, float* tag_k, void* workspace,
-                               size_t workspace_bytes, lp_stream_t stream) {
-    LP_CHECK_ARG(det && tag && val_k && ind_k && tag_k && workspace, "lp_nms_topk_f32: null pointer");
-    LP_CHECK_ARG(N > 0 && J > 0 && H > 0 && W > 0 && T > 0 && (long long)H * W < (1ll << 31),
-                 "lp_nms_topk_f32: bad shape N=%d J=%d H=%d W=%d T=%d", N, J, H, W, T);
-    LP_CHECK_ARG(K > 0 && K <= TK_MAXK, "lp_nms_topk_f32: K=%d out of range (1..%d)", K, TK_MAXK);
-    LP_CHECK_ARG(nms_kernel >= 1 && nms_kernel <= 9 && (nms_kernel & 1), "lp_nms_topk_f32: NMS kernel %d must be odd, <= 9",
-                 nms_kernel);
-    LP_CHECK_ARG((long long)N * J <= 65535, "lp_nms_topk_f32: N*J=%lld exceeds the grid limit 65535", (long long)N * J);
-    const int R = nms_kernel / 2;
-    const int sr = strip_rows(W);
-    const int nstrips = ((H + sr - 1) / sr + TK_SPB - 1) / TK_SPB;   // bands of TK_SPB strips
-    LP_CHECK_ARG(nstrips * TK_WARPS <= 256, "lp_nms_topk_f32: plane too large (H=%d W=%d)", H, W);
-    const size_t need = lp_nms_topk_workspace_bytes(N, J, H, W, K);
-    if (workspace_bytes < need) {
-        set_error("lp_nms_topk_f32: workspace %zu < required %zu bytes", workspace_bytes, need);
-        return LP_ERR_CAPACITY;
-    }
-    const size_t smem = (size_t)(sr + 2 * R) * W * sizeof(float);
-    LP_CHECK_ARG(smem <= 200 * 1024, "lp_nms_topk_f32: W=%d too wide for the strip buffers", W);
-    cudaError_t e = cudaFuncSetAttribute((const void*)nms_topk_strip_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)smem);
-    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(nms_topk)");
-    cudaStream_t s = (cudaStream_t)stream;
-    dim3 grid(nstrips, N * J);
-    unsigned long long* lists = reinterpret_cast<unsigned long long*>(workspace);
-    unsigned long long* plane_thr = lists + (size_t)N * J * nstrips * TK_WARPS * K;
-    cudaError_t em = cudaMemsetAsync(plane_thr, 0, (size_t)N * J * sizeof(unsigned long long), s);
-    if (em != cudaSuccess) return cuda_fail(em, "cudaMemsetAsync(plane_thr)");
-    // (double)v > min_value  <=>  v > floor_v with floor_v = min_value rounded DOWN to float (the reference compares the
-    // float32 values with a Python float, i.e. in double: group.py:43)
+// floor_v: (double)v > min_value  <=>  v > floor_v with floor_v = min_value rounded DOWN to float (the reference compares
+// the float32 values with a Python float, i.e. in double: group.py:43)
+static float topk_floor(double min_value) {
     float floor_v = 0.f;
     if (min_value > 0.0) {
         floor_v = (float)min_value;
         if ((double)floor_v > min_value) floor_v = nextafterf(floor_v, 0.f);
     }
-    nms_topk_strip_kernel<<<grid, TK_THREADS, smem, s>>>(det, H, W, R, sr, K, floor_v, lists, plane_thr);
+    return floor_v;
+}
+
+// Both entry points: validate, then the strip kernel over (max bands, N*J planes) and one merge warp per plane.
+static int topk_launch(const float* det, const float* tag, int N, const int32_t* hw_host, const lp_map_desc_t* desc,
+                       int J, int H, int W, int T, int nms_kernel, int K, double min_value, float* val_k, int32_t* ind_k,
+                       float* tag_k, void* workspace, size_t workspace_bytes, size_t need, lp_stream_t stream,
+                       const char* name) {
+    LP_CHECK_ARG(det && tag && val_k && ind_k && tag_k && workspace, "%s: null pointer", name);
+    LP_CHECK_ARG(K > 0 && K <= TK_MAXK, "%s: K=%d out of range (1..%d)", name, K, TK_MAXK);
+    LP_CHECK_ARG(nms_kernel >= 1 && nms_kernel <= 9 && (nms_kernel & 1), "%s: NMS kernel %d must be odd, <= 9", name,
+                 nms_kernel);
+    LP_CHECK_ARG((long long)N * J <= 65535, "%s: N*J=%lld exceeds the grid limit 65535", name, (long long)N * J);
+    const int R = nms_kernel / 2;
+    int max_bands = 0;
+    size_t smem = 0;
+    for (int n = 0; n < (hw_host ? N : 1); ++n) {
+        const int h = hw_host ? hw_host[2 * n] : H, w = hw_host ? hw_host[2 * n + 1] : W;
+        LP_CHECK_ARG(h > 0 && w > 0 && (long long)h * w < (1ll << 31), "%s: bad map size %dx%d (image %d)", name, h, w, n);
+        const int nb = plane_bands(h, w);
+        LP_CHECK_ARG(nb * TK_WARPS <= 256, "%s: plane too large (H=%d W=%d)", name, h, w);
+        const size_t sm = (size_t)(strip_rows(w) + 2 * R) * w * sizeof(float);
+        LP_CHECK_ARG(sm <= 200 * 1024, "%s: W=%d too wide for the strip buffers", name, w);
+        max_bands = nb > max_bands ? nb : max_bands;
+        smem = sm > smem ? sm : smem;
+    }
+    if (workspace_bytes < need) {
+        set_error("%s: workspace %zu < required %zu bytes", name, workspace_bytes, need);
+        return LP_ERR_CAPACITY;
+    }
+    cudaError_t e = cudaFuncSetAttribute((const void*)nms_topk_strip_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)smem);
+    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(nms_topk)");
+    cudaStream_t s = (cudaStream_t)stream;
+    const size_t planes = (size_t)N * J;
+    unsigned long long* lists = reinterpret_cast<unsigned long long*>(workspace);
+    unsigned long long* plane_thr = lists + (need - planes * sizeof(unsigned long long)) / sizeof(unsigned long long);
+    cudaError_t em = cudaMemsetAsync(plane_thr, 0, planes * sizeof(unsigned long long), s);
+    if (em != cudaSuccess) return cuda_fail(em, "cudaMemsetAsync(plane_thr)");
+    dim3 grid(max_bands, N * J);
+    nms_topk_strip_kernel<<<grid, TK_THREADS, smem, s>>>(det, desc, J, H, W, R, K, topk_floor(min_value), lists, plane_thr);
     LP_LAUNCH_CHECK("nms_topk_strip_kernel");
-    topk_merge_kernel<<<N * J, 32, 0, s>>>(lists, tag, H * W, T, nstrips * TK_WARPS, K, val_k, ind_k, tag_k);
+    topk_merge_kernel<<<N * J, 32, 0, s>>>(lists, tag, desc, J, H, W, T, K, val_k, ind_k, tag_k);
     LP_LAUNCH_CHECK("topk_merge_kernel");
     return LP_OK;
+}
+
+extern "C" size_t lp_nms_topk_workspace_bytes(int N, int J, int H, int W, int K) {
+    if (N <= 0 || J <= 0 || H <= 0 || W <= 0 || K <= 0) return 0;
+    // per-warp candidate lists + one running threshold per plane
+    return (size_t)N * topk_list_bytes(J, H, W, K) + (size_t)N * J * sizeof(unsigned long long);
+}
+
+extern "C" int lp_nms_topk_f32(const float* det, const float* tag, int N, int J, int H, int W, int T, int nms_kernel,
+                               int K, double min_value, float* val_k, int32_t* ind_k, float* tag_k, void* workspace,
+                               size_t workspace_bytes, lp_stream_t stream) {
+    LP_CHECK_ARG(N > 0 && J > 0 && H > 0 && W > 0 && T > 0 && (long long)H * W < (1ll << 31),
+                 "lp_nms_topk_f32: bad shape N=%d J=%d H=%d W=%d T=%d", N, J, H, W, T);
+    return topk_launch(det, tag, N, nullptr, nullptr, J, H, W, T, nms_kernel, K, min_value, val_k, ind_k, tag_k, workspace,
+                       workspace_bytes, lp_nms_topk_workspace_bytes(N, J, H, W, K), stream, "lp_nms_topk_f32");
+}
+
+extern "C" size_t lp_nms_topk_ragged_workspace_bytes(int N, const int32_t* hw_host, int J, int K) {
+    if (N <= 0 || !hw_host || J <= 0 || K <= 0) return 0;
+    size_t b = (size_t)N * J * sizeof(unsigned long long);
+    for (int n = 0; n < N; ++n) {
+        if (hw_host[2 * n] <= 0 || hw_host[2 * n + 1] <= 0) return 0;
+        b += topk_list_bytes(J, hw_host[2 * n], hw_host[2 * n + 1], K);
+    }
+    return b;
+}
+
+extern "C" int lp_nms_topk_ragged_f32(const float* det, const float* tag, int N, const int32_t* hw_host,
+                                      const lp_map_desc_t* desc, int J, int T, int nms_kernel, int K, double min_value,
+                                      float* val_k, int32_t* ind_k, float* tag_k, void* workspace, size_t workspace_bytes,
+                                      lp_stream_t stream) {
+    LP_CHECK_ARG(hw_host && desc, "lp_nms_topk_ragged_f32: null pointer");
+    LP_CHECK_ARG(N > 0 && J > 0 && T > 0, "lp_nms_topk_ragged_f32: bad shape N=%d J=%d T=%d", N, J, T);
+    return topk_launch(det, tag, N, hw_host, desc, J, 0, 0, T, nms_kernel, K, min_value, val_k, ind_k, tag_k, workspace,
+                       workspace_bytes, lp_nms_topk_ragged_workspace_bytes(N, hw_host, J, K), stream,
+                       "lp_nms_topk_ragged_f32");
 }

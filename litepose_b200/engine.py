@@ -8,6 +8,7 @@ C-ABI calls (include/litepose_b200.h) on NHWC fp16 activations.  A plan (buffers
 call list) is built per (N, H, W, dtype) and can be captured into a CUDA graph.
 PyTorch is used for device memory and streams only.
 """
+import collections
 import ctypes
 
 import numpy as np
@@ -27,6 +28,33 @@ def _fold(sd, bn):
 def _np16(t):
     """fp32 tensor -> contiguous uint16 view of its fp16 rounding (host)."""
     return np.ascontiguousarray(t.detach().float().cpu().half().numpy()).view(np.uint16)
+
+
+class _Bump(object):
+    """Allocator of _build_plan that carves every buffer of a plan out of one byte arena (256-byte aligned).  Without an
+    arena it only measures: the placeholders it returns have a null data pointer and the plan is thrown away."""
+
+    class _Null(object):
+        def __init__(self, shape):
+            self.shape = tuple(shape)
+
+        def data_ptr(self):
+            return 0
+
+    def __init__(self, arena=None):
+        self.arena, self.used = arena, 0
+
+    def __call__(self, shape, dtype):
+        nbytes = int(np.prod(shape)) * torch.empty((), dtype=dtype).element_size()
+        off = (self.used + 255) // 256 * 256
+        self.used = off + nbytes
+        if self.arena is None:
+            return self._Null(shape)
+        return self.arena[off:off + nbytes].view(dtype).view(shape)
+
+
+# most arena-backed plans (mixed batches) kept at once; they own no device memory of their own
+ARENA_PLANS = 16
 
 
 class _Op(object):
@@ -54,6 +82,8 @@ class LitePoseEngine(object):
                 _lib.check(self.lib.lp_device_check(), "lp_device_check")
         self.arch = arch
         self.plans = {}
+        self.arena_plans = collections.OrderedDict()    # LRU of plans whose buffers live in self.arenas
+        self.arenas = {}                                # pass -> uint8 arena shared by every arena plan of that pass
         self.use_graphs = False
         import os
         self.fuse_dw_project = os.environ.get("LP_FUSE_DW_PROJECT", "1") != "0"
@@ -242,16 +272,20 @@ class LitePoseEngine(object):
         self.P = P
 
     # ------------------------------------------------------------------ plan
-    def _build_plan(self, n, h, w, in_dtype, out_fp32, pair=False):
-        """pair: the flip test as ONE batch of 2n (images n.. are the mirrored copies, produced by the fused stem)."""
+    def _build_plan(self, n, h, w, in_dtype, out_fp32, pair=False, alloc=None):
+        """pair: the flip test as ONE batch of 2n (images n.. are the mirrored copies, produced by the fused stem).
+        alloc(shape, dtype) provides every buffer of the plan (default: a tensor of its own)."""
         if h % 16 or w % 16:
             raise ValueError("LitePose input height/width must be multiples of 16, got %dx%d" % (h, w))
         lib, P, dev = self.lib, self.P, self.device
         f16 = torch.float16
         ops = []
+        if alloc is None:
+            def alloc(shape, dtype):
+                return torch.empty(shape, dtype=dtype, device=dev)
 
         def buf(*shape):
-            return torch.empty(shape, dtype=f16, device=dev)
+            return alloc(shape, f16)
 
         plan = {"in_ptr": ctypes.c_void_p(0), "flip": ctypes.c_int(0)}
         n_in = n
@@ -291,8 +325,8 @@ class LitePoseEngine(object):
             max_e = max(max_e, e)
             max_d = max(max_d, n * th2 * tw2 * blk["dw"]["C"])
             th, tw = th2, tw2
-        e_buf = torch.empty(max_e, dtype=f16, device=dev)
-        d_buf = torch.empty(max_d, dtype=f16, device=dev)
+        e_buf = alloc((max_e,), f16)
+        d_buf = alloc((max_d,), f16)
         keep += [e_buf, d_buf]
         for blk in P["blocks"]:
             inv, dw, pc = blk["inv"], blk["dw"], blk["pc"]
@@ -342,7 +376,7 @@ class LitePoseEngine(object):
             raw = x_list[-i - 3][0]
             if i > 0:
                 hd = P["heads"][i - 1]
-                o = torch.empty((n, hd["Co"], rh, rw), dtype=torch.float32 if out_fp32 else f16, device=dev)
+                o = alloc((n, hd["Co"], rh, rw), torch.float32 if out_fp32 else f16)
                 outs.append(o)
                 if self.fuse_heads:
                     ops.append(_Op("head_fused", lib.lp_head_fused_f16,
@@ -374,6 +408,44 @@ class LitePoseEngine(object):
             self.plans[key] = pl
         return pl
 
+    @staticmethod
+    def _pass_of(flip):
+        return flip if flip == "both" else bool(flip)
+
+    def reserve_arena(self, specs):
+        """Size the arenas for the plans ``specs`` = [(n, h, w, in_dtype, out_fp32, flip)] before any of them runs.
+        An arena only grows (to the largest plan it has served); growing it drops the arena plans built on the old one.
+        Call it when nothing that reads an arena plan's buffers is still queued on another stream."""
+        need = {}
+        for n, h, w, in_dtype, out_fp32, flip in specs:
+            m = _Bump()
+            self._build_plan(n, h, w, in_dtype, out_fp32, pair=(flip == "both"), alloc=m)
+            key = self._pass_of(flip)
+            need[key] = max(need.get(key, 0), m.used)
+        for key, nbytes in need.items():
+            ar = self.arenas.get(key)
+            if ar is None or ar.numel() < nbytes:
+                for k in [k for k in self.arena_plans if k[5] == key]:
+                    del self.arena_plans[k]
+                self.arenas[key] = None
+                self.arenas[key] = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+
+    def arena_plan_for(self, n, h, w, in_dtype, out_fp32, flip=False):
+        """A plan whose buffers are carved out of the arena of its pass (plain / mirrored): plans of every size share
+        that memory, so device memory does not grow with the number of distinct (n, h, w) served.  Arena plans of one
+        pass must run in stream order (the pipeline's mixed batches do); at most ARENA_PLANS are kept."""
+        key = (n, h, w, in_dtype, out_fp32, self._pass_of(flip))
+        pl = self.arena_plans.get(key)
+        if pl is not None:
+            self.arena_plans.move_to_end(key)
+            return pl
+        self.reserve_arena([(n, h, w, in_dtype, out_fp32, flip)])
+        pl = self._build_plan(n, h, w, in_dtype, out_fp32, pair=(flip == "both"), alloc=_Bump(self.arenas[key[5]]))
+        self.arena_plans[key] = pl
+        while len(self.arena_plans) > ARENA_PLANS:
+            self.arena_plans.popitem(last=False)
+        return pl
+
     # ------------------------------------------------------------------ run
     def _launch_all(self, plan, stream_ptr):
         for op in plan["ops"]:
@@ -381,10 +453,11 @@ class LitePoseEngine(object):
             if rc:
                 _lib.check(rc, op.name)
 
-    def run(self, x, flip=False, out_fp32=True, clone=True, slot=0):
+    def run(self, x, flip=False, out_fp32=True, clone=True, slot=0, arena=False):
         """x: NCHW fp16/fp32 CUDA tensor.  Returns [out0 [N,2J,H/4,W/4], out1 [N,J,H/2,W/2]]
         (fp32 when out_fp32 else fp16).  ``flip`` computes the forward of torch.flip(x,[3]); ``flip="both"`` runs the flip test
-        as ONE batch of 2N (outputs [2N, ...]: rows N.. belong to the mirrored images)."""
+        as ONE batch of 2N (outputs [2N, ...]: rows N.. belong to the mirrored images).  ``arena``: run on an arena plan
+        (arena_plan_for; eager launches only) - its outputs are overwritten by the next arena run of the same pass."""
         if self.device.type != "cuda":
             raise RuntimeError("LitePoseEngine.run needs a CUDA device (this engine was prepared on %s)" % self.device)
         assert x.is_cuda and x.dim() == 4 and x.shape[1] == 3
@@ -392,10 +465,13 @@ class LitePoseEngine(object):
             x = x.float()
         x = x.contiguous()
         n, _, h, w = x.shape
-        plan = self.plan_for(n, h, w, x.dtype, out_fp32, flip, slot)
+        if arena:
+            plan = self.arena_plan_for(n, h, w, x.dtype, out_fp32, flip)
+        else:
+            plan = self.plan_for(n, h, w, x.dtype, out_fp32, flip, slot)
         with torch.cuda.device(self.device):
             stream = torch.cuda.current_stream().cuda_stream
-            if self.use_graphs:
+            if self.use_graphs and not arena:
                 g = plan["graph"]
                 if g is None:
                     g = plan["graph"] = {}

@@ -95,6 +95,64 @@ class DeviceParser(object):
                 b["ws_ref"].numel(), s), "lp_adjust_refine_f32")
         return b["ans"], b["num"], b["scores"]
 
+    def _ragged_buffers(self, dev, n, t, ws_topk, ws_match, ws_ref):
+        """Grow-only buffers of run_ragged: one set, sized for the largest batch seen (not one per composition)."""
+        J, K, pcap = self.J, self.K, self.pcap
+        sizes = {"val_k": (n * J * K, torch.float32), "ind_k": (n * J * K, torch.int32),
+                 "tag_k": (n * J * K * t, torch.float32), "ans": (n * pcap * J * (3 + t), torch.float32),
+                 "num": (n, torch.int32), "scores": (n * pcap, torch.float32), "ws_topk": (ws_topk, torch.uint8),
+                 "ws_match": (ws_match, torch.uint8), "ws_ref": (ws_ref, torch.uint8)}
+        bufs = self._bufs.setdefault(("ragged", dev), {})
+        out = {}
+        for name, (numel, dtype) in sizes.items():
+            b = bufs.get(name)
+            if b is None or b.numel() < numel:
+                b = bufs[name] = torch.empty(max(int(numel), 1), dtype=dtype, device=dev)
+            out[name] = b[:max(int(numel), 1)]
+        if dev not in self._jo:
+            self._jo[dev] = torch.tensor(self.joint_order, dtype=torch.int32, device=dev)
+        return out, self._jo[dev]
+
+    def workspace_bytes_ragged(self, hw, t):
+        """(top-K, matching, adjust/refine) workspace bytes of a ragged call on maps of the sizes ``hw`` [N,2]."""
+        hw = np.ascontiguousarray(hw, np.int32)
+        n = hw.shape[0]
+        return (int(self.lib.lp_nms_topk_ragged_workspace_bytes(n, hw.ctypes.data, self.J, self.K)),
+                int(self.lib.lp_tag_match_workspace_bytes(n, self.J, self.K, t, self.pcap)),
+                int(self.lib.lp_adjust_refine_workspace_bytes(n, self.J, self.pcap)))
+
+    def run_ragged(self, det, tag, hw, desc, t, adjust=True, refine=True):
+        """The parse of run() on a det / tag arena of differently sized maps: image i's [J,h_i,w_i] det block and
+        [J,h_i,w_i,T] tag block sit at the offsets of ``desc`` (device pointer to N lp_map_desc_t,
+        litepose_b200.mixed.MAP_DESC); ``hw`` [N,2] int32 host array = the same sizes.  One ragged chain (NMS/top-K, tag
+        matching, adjust/scores/refine) for the whole batch.  Per image the results equal, bit for bit, run() on that
+        image alone.  Returns device (ans [N,pcap,J,3+T], num [N], scores [N,pcap]) in grow-only buffers, valid until
+        the next ragged call."""
+        if not det.is_cuda:
+            raise RuntimeError("litepose_b200 parser runs on CUDA tensors only (no CPU fallback)")
+        hw = np.ascontiguousarray(hw, np.int32)
+        n, j = hw.shape[0], self.J
+        ws = self.workspace_bytes_ragged(hw, t)
+        with torch.cuda.device(det.device):
+            b, jo = self._ragged_buffers(det.device, n, t, *ws)
+            s = torch.cuda.current_stream().cuda_stream
+            _lib.check(self.lib.lp_nms_topk_ragged_f32(
+                det.data_ptr(), tag.data_ptr(), n, hw.ctypes.data, desc, j, t, self.nms_kernel, self.K, self.det_thr,
+                b["val_k"].data_ptr(), b["ind_k"].data_ptr(), b["tag_k"].data_ptr(), b["ws_topk"].data_ptr(),
+                b["ws_topk"].numel(), s), "lp_nms_topk_ragged_f32")
+            ans = b["ans"].view(n, self.pcap, j, 3 + t)
+            _lib.check(self.lib.lp_tag_match_ragged_f32(
+                b["val_k"].data_ptr(), b["ind_k"].data_ptr(), b["tag_k"].data_ptr(), n, j, self.K, t, desc,
+                jo.data_ptr(), self.det_thr, self.tag_thr, self.use_det_val, self.ignore_too_much, self.K,
+                self.pcap, ans.data_ptr(), b["num"].data_ptr(), b["ws_match"].data_ptr(), b["ws_match"].numel(), s),
+                "lp_tag_match_ragged_f32")
+            _lib.check(self.lib.lp_adjust_refine_ragged_f32(
+                det.data_ptr(), tag.data_ptr(), n, hw.ctypes.data, desc, j, t, self.pcap, ans.data_ptr(),
+                b["num"].data_ptr(), b["scores"].data_ptr(), 1 if adjust else 0, 1 if refine else 0,
+                b["ws_ref"].data_ptr(), b["ws_ref"].numel(), s), "lp_adjust_refine_ragged_f32")
+        self.last_ragged = b
+        return ans, b["num"], b["scores"].view(n, self.pcap)
+
     @staticmethod
     def to_reference(ans, num, scores):
         """Device results -> list over images of (ans, scores) in the reference's return

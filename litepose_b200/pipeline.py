@@ -173,13 +173,14 @@ class LitePosePipeline(object):
             for c, s in zip(*self._final)]).reshape(-1, 6))
 
     # -- device step (everything between the H2D copy and the D2H copy) -------------
-    def _network_part(self, st, x, slot=0):
-        """Both network passes -> ([o0, o1], [f0, f1]) in the engine's buffer set ``slot``."""
+    def _network_part(self, st, x, slot=0, arena=False):
+        """Both network passes -> ([o0, o1], [f0, f1]) in the engine's buffer set ``slot`` (``arena``: in the engine's
+        shared arena plans, see LitePoseEngine.arena_plan_for)."""
         eng = self.engine
         f = None
         if self.flip and self.pair_batch:
             # the flip test as ONE batch of 2N: half the launches, twice the tiles per persistent kernel
-            both = eng.run(x, flip="both", out_fp32=True, clone=False, slot=slot)
+            both = eng.run(x, flip="both", out_fp32=True, clone=False, slot=slot, arena=arena)
             nb = x.shape[0]
             o = [both[0][:nb], both[1][:nb]]
             f = [both[0][nb:], both[1][nb:]]
@@ -190,13 +191,13 @@ class LitePosePipeline(object):
             side = st["side"]
             side.wait_stream(main)
             with torch.cuda.stream(side):
-                f = eng.run(x, flip=True, out_fp32=True, clone=False, slot=slot)
-            o = eng.run(x, flip=False, out_fp32=True, clone=False, slot=slot)
+                f = eng.run(x, flip=True, out_fp32=True, clone=False, slot=slot, arena=arena)
+            o = eng.run(x, flip=False, out_fp32=True, clone=False, slot=slot, arena=arena)
             main.wait_stream(side)
         else:
-            o = eng.run(x, flip=False, out_fp32=True, clone=False, slot=slot)
+            o = eng.run(x, flip=False, out_fp32=True, clone=False, slot=slot, arena=arena)
             if self.flip:
-                f = eng.run(x, flip=True, out_fp32=True, clone=False, slot=slot)
+                f = eng.run(x, flip=True, out_fp32=True, clone=False, slot=slot, arena=arena)
         return o, f
 
     def _glue_part(self, st, o, f, det, tag):
@@ -396,16 +397,26 @@ class LitePosePipeline(object):
         big = xs[scales[0]]
         det_hw = (x1.shape[2], x1.shape[3]) if self.project else (big.shape[2] // 2, big.shape[3] // 2)
         st = self._get_state(n, x1.shape[2], x1.shape[3], x1.dtype, plant, det_hw=det_hw)
-        J = self.params.num_joints
         det, tag = st["det"], st["tag"]
         self.engine.use_graphs = False
+        self._multiscale_part(st, xs, det, tag, det_hw)
+        if st["plant"] is not None:
+            st["plant"].apply(det, tag)
+        return self._parser_part(st, det, tag, st["packed"])
+
+    def _multiscale_part(self, st, xs, det, tag, det_hw, arena=False):
+        """Per scale, largest first: both network passes and one lp_glue_scale_f32 launch accumulating into det (the
+        tags from the scale-1 pass); the last launch divides by the number of scales."""
+        scales = self.scales
+        n = det.shape[0]
+        J = self.params.num_joints
         stream = torch.cuda.current_stream().cuda_stream
         for i, s in enumerate(scales):
             x = xs[s]
             if x.shape[0] != n or x.shape[2] % 64 or x.shape[3] % 64:
                 raise ValueError("step_device_multiscale: scale %r frames %r (batch %d, sides multiples of 64 expected)"
                                  % (s, tuple(x.shape), n))
-            o, f = self._network_part(st, x)
+            o, f = self._network_part(st, x, arena=arena)
             _, _, h, w = o[0].shape
             _lib.check(self.lib.lp_glue_scale_f32(
                 o[0].data_ptr(), o[1].data_ptr(), f[0].data_ptr() if self.flip else None,
@@ -413,9 +424,6 @@ class LitePosePipeline(object):
                 1 if self.tag_shared else 0, h, w, 1 if self.flip else 0, det_hw[0], det_hw[1], 1 if i > 0 else 0,
                 float(len(scales)) if i == len(scales) - 1 else 1.0,
                 det.data_ptr(), tag.data_ptr() if s == 1.0 else None, stream), "lp_glue_scale_f32")
-        if st["plant"] is not None:
-            st["plant"].apply(det, tag)
-        return self._parser_part(st, det, tag, st["packed"])
 
     def step_multiscale(self, frames, plant=None):
         """Public blocking call of the multi-scale test: {scale: pinned host frames} in, host result out (the list
@@ -436,7 +444,13 @@ class LitePosePipeline(object):
         resize_align_multi_scale + ToTensor + Normalize on the device (lp_warp_affine_normalize_u8) -> the network
         passes, glue and parser of step() / step_multiscale() -> get_final_preds on the device.  Returns the list over
         images of (final_results [P,J,3+T] in the coordinates of the original image, scores, P) - per image what
-        valid.py:227-233 holds in ``final_results`` and ``scores``."""
+        valid.py:227-233 holds in ``final_results`` and ``scores``.
+
+        ``images`` may also be a LIST of uint8 [H_i,W_i,3] images (numpy arrays or tensors) of any sizes - a real
+        evaluation set, where every image has its own network size (infer_mixed); ``plant`` is then a list with one
+        batch-1 PlantedCrowd or None per image."""
+        if isinstance(images, (list, tuple)):
+            return self.infer_mixed(images, mean, std, half, plant)
         import numpy as np
         from .lib.utils import transforms as T
         if images.dim() != 4 or images.shape[3] != 3 or images.dtype != torch.uint8:
@@ -469,6 +483,134 @@ class LitePosePipeline(object):
                 self.set_final_preds(None)
             else:
                 self.set_final_preds(prev[0], prev[1])
+
+    # -- mixed batches: differently sized images in one call --------------------------------------------------------
+    def _grow(self, name, numel, dtype, pinned=False):
+        """Grow-only buffer of the mixed path (``numel`` elements at least): its size follows the largest batch served,
+        not the number of batch compositions."""
+        buf = self._mixed_bufs.get(name)
+        if buf is None or buf.numel() < numel or buf.dtype != dtype:
+            if pinned:
+                buf = torch.empty(max(int(numel), 1), dtype=dtype).pin_memory()
+            else:
+                buf = torch.empty(max(int(numel), 1), dtype=dtype, device=self.device)
+            self._mixed_bufs[name] = buf
+        return buf[:numel]
+
+    def infer_mixed(self, images, mean=(0.485, 0.456, 0.406), std=(0.229, 0.224, 0.225), half=True, plant=None):
+        """infer_images for a list of uint8 [H_i,W_i,3] images of any sizes.  Per image the result equals, bit for bit,
+        infer_images(image[None]); the list comes back in the caller's order.  The images are grouped by their per-scale
+        network sizes (litepose_b200.mixed.MixedPlan).  Once per batch: one H2D copy of the packed images and
+        descriptors, per scale ONE ragged warp launch (lp_warp_affine_normalize_ragged_u8) into the input arena of that
+        scale; per size group the network passes and the glue on the existing kernels (arena plans of the engine: their
+        activation memory is shared by every group size), writing the group's slice of the det / tag arena; then ONE
+        ragged parser chain over the whole arena, one get_final_preds launch with per-image matrices, one payload pack
+        and one D2H copy.  Launches run eagerly (no CUDA graph: the composition changes from batch to batch)."""
+        import numpy as np
+        from .mixed import MixedPlan, image_shapes
+        shapes = image_shapes(images)
+        n = len(shapes)
+        if plant is not None and len(plant) != n:
+            raise ValueError("infer_images: %d plant entries for %d images" % (len(plant), n))
+        J = self.params.num_joints
+        T = 2 if self.flip else 1
+        mp = MixedPlan(shapes, self.scales, int(self.cfg.DATASET.INPUT_SIZE), self.project, J, T)
+        if not hasattr(self, "_mixed_bufs"):
+            self._mixed_bufs = {}
+            self._mixed_side = torch.cuda.Stream(device=self.device, priority=self.prio_net)
+        dev = self.device
+        in_dtype = torch.float16 if half else torch.float32
+        main = torch.cuda.current_stream()
+        # (1) one pinned staging buffer: the images (arena order) followed by the descriptors and final-pred matrices
+        descs = [mp.warp_desc(s).view(np.uint8) for s in self.scales]
+        mdesc = mp.map_desc().view(np.uint8)
+        trans = np.ascontiguousarray(mp.final_trans()).reshape(-1).view(np.uint8)
+        blobs = descs + [mdesc, trans]
+        img_bytes = int(mp.src_off[-1])
+        offs, o = [], (img_bytes + 255) // 256 * 256
+        for b in blobs:
+            offs.append(o)
+            o = (o + b.size + 255) // 256 * 256
+        host = self._grow("stage", o, torch.uint8, pinned=True)
+        hnp = host.numpy()
+        dev_imgs = []
+        for p, i in enumerate(mp.order):
+            im = images[i]
+            a, b = int(mp.src_off[p]), int(mp.src_off[p + 1])
+            if torch.is_tensor(im) and im.is_cuda:
+                dev_imgs.append((a, b, im))
+            else:
+                hnp[a:b] = (im.contiguous().numpy() if torch.is_tensor(im) else np.ascontiguousarray(im)).reshape(-1)
+        for b, off in zip(blobs, offs):
+            hnp[off:off + b.size] = b
+        d = self._grow("stage_dev", o, torch.uint8)
+        d.copy_(host, non_blocking=True)
+        for a, b, im in dev_imgs:                    # images already on the device: one device copy each
+            d[a:b].copy_(im.reshape(-1))
+        # (2) per scale one ragged warp + ToTensor + Normalize into the scale's input arena
+        mean_a, std_a = np.asarray(mean, np.float32), np.asarray(std, np.float32)
+        xs_arena = {}
+        stream = main.cuda_stream
+        for k, s in enumerate(self.scales):
+            xa = self._grow("x%d" % k, int(mp.in_off[s][-1]), in_dtype)
+            mh, mw = mp.max_in_hw(s)
+            _lib.check(self.lib.lp_warp_affine_normalize_ragged_u8(
+                d.data_ptr(), n, d.data_ptr() + offs[k], mw, mh, mean_a.ctypes.data, std_a.ctypes.data, xa.data_ptr(),
+                2 if half else 1, stream), "lp_warp_affine_normalize_ragged_u8")
+            xs_arena[s] = xa
+        # (3) per size group: the network passes + glue on the existing kernels, into the group's arena slice
+        det_a = self._grow("det", int(mp.det_off[-1]), torch.float32)
+        tag_a = self._grow("tag", int(mp.tag_off[-1]), torch.float32)
+        self.engine.use_graphs = False
+        specs = []
+        for g in mp.groups:
+            for s in self.scales:
+                hs, ws = g.in_hw[s]
+                if self.flip and self.pair_batch:
+                    specs.append((g.n, hs, ws, in_dtype, True, "both"))
+                else:
+                    specs.append((g.n, hs, ws, in_dtype, True, False))
+                    if self.flip:
+                        specs.append((g.n, hs, ws, in_dtype, True, True))
+        self.engine.reserve_arena(specs)
+        st = {"side": self._mixed_side, "plant": None}
+        for g in mp.groups:
+            p0, p1 = g.start, g.start + g.n
+            hd, wd = g.det_hw
+            det = det_a[int(mp.det_off[p0]):int(mp.det_off[p1])].view(g.n, J, hd, wd)
+            tag_full = tag_a[int(mp.tag_off[p0]):int(mp.tag_off[p1])].view(g.n, J, hd, wd, T)
+            tag = self._grow("tag_shared", g.n * hd * wd * T, torch.float32).view(g.n, 1, hd, wd, T) \
+                if self.tag_shared else tag_full
+            xs = {s: xs_arena[s][int(mp.in_off[s][p0]):int(mp.in_off[s][p1])].view(g.n, 3, *g.in_hw[s])
+                  for s in self.scales}
+            if len(self.scales) == 1:
+                o, f = self._network_part(st, xs[1.0], arena=True)
+                self._glue_part(st, o, f, det, tag)
+            else:
+                self._multiscale_part(st, xs, det, tag, g.det_hw, arena=True)
+            if plant is not None:
+                for k, i in enumerate(g.images):
+                    if plant[i] is not None:
+                        plant[i].apply(det[k:k + 1], tag[k:k + 1])
+            if self.tag_shared:
+                tag_full.copy_(tag.expand(-1, J, -1, -1, -1))
+        # (4) once per batch: ragged parser, get_final_preds, payload, D2H
+        hw = np.ascontiguousarray(mp.det_hw, np.int32)
+        ans, num, scores = self.parser.run_ragged(det_a, tag_a, hw, d[offs[-2]:].data_ptr(), T, self.adjust, self.refine)
+        pcap = ans.shape[1]
+        _lib.check(self.lib.lp_transform_preds_f32(ans.data_ptr(), num.data_ptr(), d.data_ptr() + offs[-1], n, pcap, J,
+                                                   ans.shape[3], stream), "lp_transform_preds_f32")
+        row = J * (3 + T)
+        width = self.keep * row + self.keep + 1
+        packed = self._grow("packed", n * width, torch.float32).view(n, width)
+        _lib.check(self.lib.lp_pack_payload_f32(ans.data_ptr(), num.data_ptr(), scores.data_ptr(), n, pcap, row,
+                                                self.keep, packed.data_ptr(), stream), "lp_pack_payload_f32")
+        out_h = self._grow("host", n * width, torch.float32, pinned=True).view(n, width)
+        out_h.copy_(packed, non_blocking=True)
+        main.synchronize()
+        res = self.unpack(out_h, row, T, self.fetch_overflow({"full": (ans, num, scores)}, out_h))
+        self._last_mixed = {"plan": mp, "det": det_a, "tag": tag_a, "inputs": xs_arena}
+        return [res[int(p)] for p in mp.pos]
 
     # -- asynchronous end-to-end API: two steps in flight -----------------------------------------
     def submit(self, frames_pinned, plant=None, group=None, dst=0):

@@ -25,6 +25,8 @@ def parse_args(argv=None):
     ap.add_argument("--images", type=int, default=8, help="batch of equally sized synthetic images")
     ap.add_argument("--height", type=int, default=480)
     ap.add_argument("--width", type=int, default=640)
+    ap.add_argument("--sizes", default=None, metavar="HxW,HxW,...",
+                    help="a mixed list of image sizes (one image each) instead of --images x --height x --width")
     ap.add_argument("--repeat", type=int, default=5)
     ap.add_argument("--dry-run", action="store_true")
     ap.add_argument("opts", nargs=argparse.REMAINDER, help="KEY VALUE pairs, as valid.py takes them")
@@ -39,10 +41,19 @@ def main(argv=None):
     if arch is None:
         raise SystemExit("--superconfig is required for pose_mobilenet (valid.py:106-111)")
     LitePosePipeline._validate_cfg(cfg)
+    sizes = None
+    if args.sizes:
+        try:
+            sizes = [tuple(int(v) for v in s.lower().split("x")) for s in args.sizes.split(",")]
+        except ValueError:
+            raise SystemExit("--sizes: HxW,HxW,... expected, got %r" % args.sizes)
+        if any(len(s) != 2 or min(s) <= 0 for s in sizes):
+            raise SystemExit("--sizes: HxW,HxW,... expected, got %r" % args.sizes)
     summary = {"model": cfg.MODEL.NAME, "input_size": cfg.DATASET.INPUT_SIZE, "joints": cfg.DATASET.NUM_JOINTS,
                "scale_factor": list(cfg.TEST.SCALE_FACTOR), "flip_test": cfg.TEST.FLIP_TEST,
                "project2image": cfg.TEST.PROJECT2IMAGE, "fp16": cfg.FP16.ENABLED, "adjust": cfg.TEST.ADJUST,
-               "refine": cfg.TEST.REFINE, "images": [args.images, args.height, args.width, 3]}
+               "refine": cfg.TEST.REFINE,
+               "images": [args.images, args.height, args.width, 3] if sizes is None else [[h, w, 3] for h, w in sizes]}
     if args.dry_run:
         print(json.dumps(summary))
         return summary
@@ -57,15 +68,18 @@ def main(argv=None):
         model.load_state_dict(torch.load(cfg.TEST.MODEL_FILE, map_location="cpu"), strict=True)
     model = model.cuda().eval()       # FP16.ENABLED: the frames are fed as fp16 (what tofp16 does, fp16util.py:40-47); the
     pipe = LitePosePipeline(model, cfg)   # engine computes in fp16 with BN folded in fp32 either way (DESIGN.md 3)
-    imgs = torch.from_numpy(np.random.RandomState(0).randint(0, 256, (args.images, args.height, args.width, 3))
-                            .astype(np.uint8)).pin_memory()
+    rng = np.random.RandomState(0)
+    if sizes is None:
+        imgs = torch.from_numpy(rng.randint(0, 256, (args.images, args.height, args.width, 3)).astype(np.uint8)).pin_memory()
+    else:                             # a mixed list: one infer_images call on images of different sizes
+        imgs = [rng.randint(0, 256, (h, w, 3)).astype(np.uint8) for h, w in sizes]
     res = pipe.infer_images(imgs, half=bool(cfg.FP16.ENABLED))
     torch.cuda.synchronize()
     t0 = time.perf_counter()
     for _ in range(args.repeat):
         res = pipe.infer_images(imgs, half=bool(cfg.FP16.ENABLED))
     dt = (time.perf_counter() - t0) / args.repeat
-    summary.update({"persons": [r[2] for r in res], "frames_per_s": args.images / dt, "ms_per_batch": dt * 1e3})
+    summary.update({"persons": [r[2] for r in res], "frames_per_s": len(imgs) / dt, "ms_per_batch": dt * 1e3})
     print(json.dumps(summary))
     return summary
 
