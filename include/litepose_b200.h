@@ -296,6 +296,22 @@ int lp_assign_f32(const int32_t* count, const float* val, const float* tag, cons
                   const int32_t* joint_order, int N, int C, int M, float threshold,
                   int32_t* num_person, float* ans, int32_t* status, lp_stream_t stream);
 
+/* lp_find_peaks_f32 on the maps as the glue writes them, uniform or ragged, in ONE launch
+ * (the pipeline's fast grouping mode).  det [N,J,H,W] f32, or image n's [J,h,w] block at
+ * desc[n].det_offset; the tag of a peak is read IN PLACE at channel 0 of the interleaved
+ * [N,tag_planes,H,W,T] map (or image n's [tag_planes,h,w,T] block at desc[n].tag_offset).
+ * tag_planes: J, or 1 = one map shared by every joint (MODEL.TAG_PER_JOINT off).
+ * Uniform: hw_host = desc = NULL.  Ragged: hw_host [N][2] (HOST) = the (h, w) of desc (device),
+ * H and W are ignored.  One CTA per (image, joint) plane, N*J planes.  Outputs as for
+ * lp_find_peaks_f32 (count [N,J], val/tag_out [N,J,M], ind [N,J,M,2]; entries past count
+ * untouched) and per image bit-identical to lp_find_peaks_f32 on det[n] and
+ * tag[n,...,0].contiguous(): the same device code. */
+int lp_find_peaks_maps_f32(const float* det, const float* tag, int N, int H, int W,
+                           const int32_t* hw_host, const lp_map_desc_t* desc, int J, int T,
+                           int tag_planes, int M, float threshold, int window_size,
+                           int32_t* count, float* val, float* tag_out, int32_t* ind,
+                           lp_stream_t stream);
+
 /* ---- glue ("next" row 1): fused flip/upsample/average/project ----------------
  * From the two forward passes' outputs (plain: o0 [N,2J,h,w], o1 [N,J,2h,2w]; flipped
  * pass: f0, f1, NULL when flip == 0) produce det [N,J,Hd,Wd] and tag [N,J,Hd,Wd,T]
@@ -337,6 +353,10 @@ int lp_glue_scale_f32(const float* o0, const float* o1, const float* f0, const f
  * caller then fetches the image from the parser's buffers - nothing is clipped silently). */
 int lp_pack_payload_f32(const float* ans, const int32_t* num_people, const float* scores, int N,
                         int pcap, int row, int keep, float* packed, lp_stream_t stream);
+/* The fast grouping's row per image: packed [N, M*C*4 + 2] f32 = ans [N,M,C,4] of
+ * lp_assign_f32 (every person: M <= 32) | person count | KM status (0 ok, 1 round cap hit). */
+int lp_pack_fast_payload_f32(const float* ans, const int32_t* num_person, const int32_t* status,
+                             int N, int M, int C, float* packed, lp_stream_t stream);
 
 /* ---- synthetic workload: planted persons (bench / tests only) --------------------
  * A random-weight network detects nobody, so the benchmark plants persons between glue and

@@ -80,6 +80,8 @@ SIGNATURES = {
     "lp_transform_preds_f32": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "lp_find_peaks_f32": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _f, _i, _vp, _vp, _vp, _vp, _vp]),
     "lp_assign_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _f, _vp, _vp, _vp, _vp]),
+    "lp_find_peaks_maps_f32": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _i, _i, _i, _i, _f, _i, _vp, _vp, _vp, _vp, _vp]),
+    "lp_pack_fast_payload_f32": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp]),
 }
 
 _lock = threading.Lock()

@@ -38,18 +38,14 @@ __device__ __forceinline__ bool fu_is_peak(const float* __restrict__ in, int idx
     return peak;
 }
 
-__global__ void __launch_bounds__(FP_THREADS)
-find_peaks_kernel(const float* __restrict__ input, const float* __restrict__ tmap, int H, int W, int M, float thr,
-                  int window_size, int* __restrict__ count, float* __restrict__ val, float* __restrict__ tag,
-                  int* __restrict__ ind) {
+// One (image, joint) plane, one CTA: `in` is the H x W heat-map, the tag of pixel idx is tm[idx * tstride] (1: a plain
+// [H,W] map; T: channel 0 of an interleaved [H,W,T] map).  Writes count[0] and the first min(count, M) entries of
+// pv / pt / pi; entries past the count are not written.
+__device__ __forceinline__ void fu_find_peaks_plane(const float* __restrict__ in, const float* __restrict__ tm, int H, int W,
+                                                    int tstride, int M, float thr, int window_size, int* __restrict__ count,
+                                                    float* __restrict__ pv, float* __restrict__ pt, int* __restrict__ pi) {
     __shared__ int s_warp[FP_THREADS / 32];
-    const int plane = blockIdx.x;
     const int HW = H * W;
-    const float* in = input + (size_t)plane * HW;
-    const float* tm = tmap + (size_t)plane * HW;
-    float* pv = val + (size_t)plane * M;
-    float* pt = tag + (size_t)plane * M;
-    int* pi = ind + (size_t)plane * M * 2;
     const int win = window_size / 2;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     int base = 0;     // peaks found before this chunk (identical in every thread)
@@ -87,14 +83,50 @@ find_peaks_kernel(const float* __restrict__ input, const float* __restrict__ tma
                     pi[2 * r] = idx - i * W;
                     pi[2 * r + 1] = i;
                     pv[r] = in[idx];
-                    pt[r] = tm[idx];
+                    pt[r] = tm[(size_t)idx * tstride];
                 }
                 ++r;
             }
         base += total;
         __syncthreads();
     }
-    if (threadIdx.x == 0) count[plane] = min(base, M);
+    if (threadIdx.x == 0) *count = min(base, M);
+}
+
+__global__ void __launch_bounds__(FP_THREADS)
+find_peaks_kernel(const float* __restrict__ input, const float* __restrict__ tmap, int H, int W, int M, float thr,
+                  int window_size, int* __restrict__ count, float* __restrict__ val, float* __restrict__ tag,
+                  int* __restrict__ ind) {
+    const int plane = blockIdx.x;
+    const size_t HW = (size_t)H * W;
+    fu_find_peaks_plane(input + plane * HW, tmap + plane * HW, H, W, 1, M, thr, window_size, count + plane,
+                        val + (size_t)plane * M, tag + (size_t)plane * M, ind + (size_t)plane * M * 2);
+}
+
+// The same planes read where the pipeline's glue leaves them: det [N,J,H,W] (or image n's [J,h,w] block at
+// desc[n].det_offset), tag [N,tag_planes,H,W,T] (or [tag_planes,h,w,T] at desc[n].tag_offset) read in place at channel
+// 0; tag_planes == 1 serves every joint from the one shared map.  Outputs in the layouts of find_peaks_kernel.
+// (The minimum of 4 resident CTAs lifts ptxas' default 32-register budget, which spills the tag stride here.)
+__global__ void __launch_bounds__(FP_THREADS, 4)
+find_peaks_maps_kernel(const float* __restrict__ det, const float* __restrict__ tmap, const lp_map_desc_t* __restrict__ desc,
+                       int J, int H, int W, int T, int tag_planes, int M, float thr, int window_size,
+                       int* __restrict__ count, float* __restrict__ val, float* __restrict__ tag, int* __restrict__ ind) {
+    const int plane = blockIdx.x;
+    const int n = plane / J, j = plane - n * J;
+    const int tj = tag_planes == 1 ? 0 : j;
+    int h = H, w = W;
+    size_t det_off, tag_off;
+    if (desc == nullptr) {
+        det_off = (size_t)plane * H * W;
+        tag_off = ((size_t)n * tag_planes + tj) * H * W * T;
+    } else {
+        h = desc[n].h;
+        w = desc[n].w;
+        det_off = (size_t)desc[n].det_offset + (size_t)j * h * w;
+        tag_off = (size_t)desc[n].tag_offset + (size_t)tj * h * w * T;
+    }
+    fu_find_peaks_plane(det + det_off, tmap + tag_off, h, w, T, M, thr, window_size, count + plane,
+                        val + (size_t)plane * M, tag + (size_t)plane * M, ind + (size_t)plane * M * 2);
 }
 
 // ---------------------------------------------------------------------------------------------- assign
@@ -394,6 +426,29 @@ extern "C" int lp_find_peaks_f32(const float* input, const float* tmap, int N, i
     find_peaks_kernel<<<N * C, FP_THREADS, 0, (cudaStream_t)stream>>>(input, tmap, H, W, M, threshold, window_size, count,
                                                                       val, tag, ind);
     LP_LAUNCH_CHECK("find_peaks_kernel");
+    return LP_OK;
+}
+
+extern "C" int lp_find_peaks_maps_f32(const float* det, const float* tag, int N, int H, int W, const int32_t* hw_host,
+                                      const lp_map_desc_t* desc, int J, int T, int tag_planes, int M, float threshold,
+                                      int window_size, int32_t* count, float* val, float* tag_out, int32_t* ind,
+                                      lp_stream_t stream) {
+    LP_CHECK_ARG(det && tag && count && val && tag_out && ind, "lp_find_peaks_maps_f32: null pointer");
+    LP_CHECK_ARG((hw_host == nullptr) == (desc == nullptr), "lp_find_peaks_maps_f32: hw_host and desc go together");
+    LP_CHECK_ARG(N > 0 && J > 0 && T > 0 && M > 0 && window_size >= 0 && (tag_planes == 1 || tag_planes == J) &&
+                     (long long)N * J <= 0x7fffffffll,
+                 "lp_find_peaks_maps_f32: bad shape N=%d J=%d T=%d tag_planes=%d M=%d window=%d", N, J, T, tag_planes, M,
+                 window_size);
+    // one CTA per plane whatever its size: the host sizes only validate the planes
+    for (int n = 0; n < (hw_host ? N : 1); ++n) {
+        const int h = hw_host ? hw_host[2 * n] : H, w = hw_host ? hw_host[2 * n + 1] : W;
+        LP_CHECK_ARG(h > 0 && w > 0 && (long long)h * w <= 0x7fffffffll, "lp_find_peaks_maps_f32: bad map size %dx%d "
+                     "(image %d)", h, w, n);
+    }
+    find_peaks_maps_kernel<<<N * J, FP_THREADS, 0, (cudaStream_t)stream>>>(det, tag, desc, J, H, W, T, tag_planes, M,
+                                                                           threshold, window_size, count, val, tag_out,
+                                                                           ind);
+    LP_LAUNCH_CHECK("find_peaks_maps_kernel");
     return LP_OK;
 }
 

@@ -6,6 +6,9 @@
 // HeatmapParser.parse returns to valid.py:227 (reference lib/core/group.py:269-291) in a form one D2H copy / one NCCL
 // gather can carry.  One launch instead of three strided torch copies.
 //
+// lp_pack_fast_payload_f32: the same for the fast grouping (find_peaks + KM assign, fast_utils.cu): every one of the
+// at most M <= 32 persons (ans [N,M,C,4]), the person count and the KM status - no overflow path is needed.
+//
 // lp_plant_crowd_f32: a random-weight network detects nobody (SURVEY H8), so the benchmark plants persons into the
 // projected maps between glue and parser: Gaussian patches max-composited into det (order independent), tag patches
 // overwriting tag.  Index / value lists are built once on the host (litepose_b200.pipeline.PlantedCrowd).
@@ -25,6 +28,20 @@ pack_payload_kernel(const float* __restrict__ ans, const int32_t* __restrict__ n
     else if (e < keep * row + keep) v = scores[(size_t)n * pcap + (e - keep * row)];
     else v = (float)num[n];
     packed[(size_t)n * width + e] = v;
+}
+
+// the fast grouping's row: M*C*4 keypoint floats | person count | KM status
+__global__ void __launch_bounds__(256)
+pack_fast_payload_kernel(const float* __restrict__ ans, const int32_t* __restrict__ num,
+                         const int32_t* __restrict__ status, int kp, float* __restrict__ packed) {
+    const int n = blockIdx.y;
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= kp + 2) return;
+    float v;
+    if (e < kp) v = ans[(size_t)n * kp + e];
+    else if (e == kp) v = (float)num[n];
+    else v = (float)status[n];
+    packed[(size_t)n * (kp + 2) + e] = v;
 }
 
 __device__ __forceinline__ void atomic_max_f32(float* addr, float v) {
@@ -57,6 +74,18 @@ extern "C" int lp_pack_payload_f32(const float* ans, const int32_t* num_people, 
     dim3 grid((unsigned)((width + 255) / 256), N);
     pack_payload_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(ans, num_people, scores, pcap, row, keep, packed);
     LP_LAUNCH_CHECK("pack_payload_kernel");
+    return LP_OK;
+}
+
+extern "C" int lp_pack_fast_payload_f32(const float* ans, const int32_t* num_person, const int32_t* status, int N, int M,
+                                        int C, float* packed, lp_stream_t stream) {
+    LP_CHECK_ARG(ans && num_person && status && packed, "lp_pack_fast_payload_f32: null pointer");
+    LP_CHECK_ARG(N > 0 && N <= 65535 && M > 0 && C > 0 && (long long)M * C * 4 + 2 < (1ll << 30),
+                 "lp_pack_fast_payload_f32: bad shape N=%d M=%d C=%d", N, M, C);
+    const int kp = M * C * 4;
+    dim3 grid((unsigned)((kp + 2 + 255) / 256), N);
+    pack_fast_payload_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(ans, num_person, status, kp, packed);
+    LP_LAUNCH_CHECK("pack_fast_payload_kernel");
     return LP_OK;
 }
 

@@ -87,11 +87,40 @@ class PlantedCrowd(object):
         return det, tag
 
 
+def unpack_fast_payload(host, M, J):
+    """Rows of lp_pack_fast_payload_f32 ([N, M*J*4 + 2] float32 host tensor or array: M persons x J joints x (x, y,
+    val, tag) | person count | KM status) -> list over images of (ans ndarray [P,J,4], P).  Raises LitePoseError on an
+    image whose KM assignment hit its round cap (status 1): such a result is never returned."""
+    import numpy as np
+    a = host.numpy() if torch.is_tensor(host) else np.asarray(host, np.float32)
+    kp = M * J * 4
+    if a.ndim != 2 or a.shape[1] != kp + 2:
+        raise ValueError("fast payload: rows of %d floats expected, got shape %r" % (kp + 2, a.shape))
+    out = []
+    for i in range(a.shape[0]):
+        if int(a[i, kp + 1]) != 0:
+            raise _lib.LitePoseError("image %d: the KM assignment hit its round cap (status %d); no result"
+                                     % (i, int(a[i, kp + 1])))
+        p = int(a[i, kp])
+        out.append((a[i, :kp].reshape(M, J, 4)[:p].copy(), p))
+    return out
+
+
 class LitePosePipeline(object):
-    def __init__(self, model, cfg, use_graphs=True, keep=64):
-        """model: litepose_b200 drop-in LitePose on a CUDA device (eval)."""
+    def __init__(self, model, cfg, use_graphs=True, keep=64, grouping="ae"):
+        """model: litepose_b200 drop-in LitePose on a CUDA device (eval).
+
+        grouping: "ae" - the evaluation parser (lib/core/group.py: NMS/top-K, tag matching, adjust, refine, scores);
+        "fast" - the demo's parser (nano_demo/fast_utils/group.py:38-47: peak finder + KM assignment, no adjust /
+        refine, at most 32 persons).  Every entry point then returns, per image, (ans [P,J,4] float32 = x, y, val, tag
+        in person-creation order, P) instead of (ans [P,J,3+T], scores, P)."""
+        if grouping not in ("ae", "fast"):
+            raise ValueError("grouping=%r: 'ae' or 'fast' expected" % (grouping,))
         self.cfg = cfg
         self._validate_cfg(cfg)
+        self.grouping = grouping
+        if grouping == "fast":
+            self._validate_fast_cfg(cfg)
         self.lib = _lib.load()
         self.device = next(model.parameters()).device
         self.engine = model.lp_engine(self.device)
@@ -125,6 +154,16 @@ class LitePosePipeline(object):
         # never clipped: step() fetches the full result from the parser's buffers (capacity J*K persons) in a second
         # copy, and unpack() raises if it is handed an overflowing payload without that second copy.
         self.keep = min(int(keep), self.parser.pcap)
+        if grouping == "fast":
+            from .fast_utils.group import Params as FastParams
+            fp = FastParams(cfg)
+            J = p.num_joints
+            # the demo's parser hands joint_order to assign(), which reads the first C entries: the entries that name no
+            # plane are dropped, as fast_utils.group.HeatmapParser._joint_order does
+            self.fast = {"M": int(fp.max_num_people), "thr": float(fp.detection_threshold), "win": int(fp.window_size),
+                         "tag_thr": float(fp.tag_threshold),
+                         "jo": torch.tensor([j for j in fp.joint_order if j < J][:J], dtype=torch.int32,
+                                            device=self.device)}
         self._state = {}
         self._async = None                # submit()/collect() slots
         self._final = None                # per-image inverse affines of get_final_preds (host, [N,6] float64)
@@ -153,6 +192,22 @@ class LitePosePipeline(object):
             bad("WITH_AE_LOSS / TEST.WITH_AE other than (True, False)")
         if int(cfg.LOSS.NUM_STAGES) != 2:
             bad("LOSS.NUM_STAGES=%r" % (cfg.LOSS.NUM_STAGES,))
+
+    @staticmethod
+    def _validate_fast_cfg(cfg):
+        """grouping="fast" runs the demo's parser as it is (nano_demo/fast_utils/group.py:38-47): peaks + KM assignment,
+        nothing else.  Settings it cannot honour are refused, not ignored: adjust / refine (the demo's cfg turns both
+        off, nano_demo/core/__init__.py:106-116) and more than 32 persons (the KM kernel holds 32 per joint)."""
+        why = []
+        if int(cfg.DATASET.MAX_NUM_PEOPLE) > 32:
+            why.append("DATASET.MAX_NUM_PEOPLE=%d exceeds the 32 persons the KM assignment holds"
+                       % int(cfg.DATASET.MAX_NUM_PEOPLE))
+        if cfg.TEST.ADJUST:
+            why.append("TEST.ADJUST is on (the fast parser has no adjust step)")
+        if cfg.TEST.REFINE:
+            why.append("TEST.REFINE is on (the fast parser has no refine step)")
+        if why:
+            raise ValueError("LitePosePipeline(grouping='fast'): " + "; ".join(why))
 
     def set_final_preds(self, centers=None, scales=None):
         """valid.py:230-233 on the device: after this call every step maps the keypoints of image i back to its original
@@ -227,6 +282,8 @@ class LitePosePipeline(object):
     def _parser_part(self, st, det, tag, packed):
         """Device parser (+ get_final_preds) on det / tag -> packed fixed-size payload."""
         n = det.shape[0]
+        if self.grouping == "fast":
+            return self._fast_parser_part(st, det, tag, packed)
         if self.tag_shared:
             # MODEL.TAG_PER_JOINT off: the one tag map serves every joint (group.py:150-152); the parser kernels index
             # [N,J,H,W,T], so the map is tiled here (one strided copy; not the shipped configuration)
@@ -241,6 +298,55 @@ class LitePosePipeline(object):
                                                 st["row"], self.keep, packed.data_ptr(),
                                                 torch.cuda.current_stream().cuda_stream), "lp_pack_payload_f32")
         return packed
+
+    def _fast_buffers(self, n, J, alloc=None):
+        """Peaks, persons and status of the fast grouping for n images; ``alloc(name, shape, dtype)`` (default: new
+        device tensors) lets the mixed path serve them from its grow-only buffers."""
+        if alloc is None:
+            alloc = lambda name, shape, dt: torch.empty(shape, dtype=dt, device=self.device)
+        f32, i32, M = torch.float32, torch.int32, self.fast["M"]
+        spec = {"count": ((n, J), i32), "val": ((n, J, M), f32), "tag": ((n, J, M), f32), "ind": ((n, J, M, 2), i32),
+                "ans": ((n, M, J, 4), f32), "num": ((n,), i32), "status": ((n,), i32)}
+        return {k: alloc(k, shape, dt) for k, (shape, dt) in spec.items()}
+
+    def _fast_parse(self, b, det, tag, n, J, T, tag_planes, hw, desc, trans, packed):
+        """The demo's parser on det / tag where the glue left them: zero ans, find peaks (tag channel 0 read in place),
+        KM assignment, get_final_preds (``trans``: device [N,6] float64 or None), pack.  Uniform maps: ``hw`` / ``desc``
+        None, det [N,J,H,W]; ragged arena: ``hw`` [N,2] host int32 and ``desc`` the device lp_map_desc_t pointer."""
+        f, M = self.fast, self.fast["M"]
+        s = torch.cuda.current_stream().cuda_stream
+        ans = b["ans"]
+        # lp_assign_f32 writes only the entries it assigns: without this the rows of the previous step would remain
+        ans.zero_()
+        H, W = (det.shape[2], det.shape[3]) if desc is None else (0, 0)
+        _lib.check(self.lib.lp_find_peaks_maps_f32(
+            det.data_ptr(), tag.data_ptr(), n, H, W, None if hw is None else hw.ctypes.data, desc, J, T, tag_planes, M,
+            f["thr"], f["win"], b["count"].data_ptr(), b["val"].data_ptr(), b["tag"].data_ptr(), b["ind"].data_ptr(), s),
+            "lp_find_peaks_maps_f32")
+        _lib.check(self.lib.lp_assign_f32(b["count"].data_ptr(), b["val"].data_ptr(), b["tag"].data_ptr(),
+                                          b["ind"].data_ptr(), f["jo"].data_ptr(), n, J, M, f["tag_thr"],
+                                          b["num"].data_ptr(), ans.data_ptr(), b["status"].data_ptr(), s), "lp_assign_f32")
+        if trans is not None:
+            _lib.check(self.lib.lp_transform_preds_f32(ans.data_ptr(), b["num"].data_ptr(), trans, n, M, J, 4, s),
+                       "lp_transform_preds_f32")
+        _lib.check(self.lib.lp_pack_fast_payload_f32(ans.data_ptr(), b["num"].data_ptr(), b["status"].data_ptr(), n, M,
+                                                     J, packed.data_ptr(), s), "lp_pack_fast_payload_f32")
+        return packed
+
+    def _fast_parser_part(self, st, det, tag, packed):
+        n, J = det.shape[0], det.shape[1]
+        trans = st["trans"].data_ptr() if st["trans"] is not None else None
+        return self._fast_parse(st["fast"], det, tag, n, J, tag.shape[4], tag.shape[1], None, None, trans, packed)
+
+    def unpack_fast(self, host):
+        """Fast-grouping payload (host) -> list over images of (ans ndarray [P,J,4], P); see unpack_fast_payload."""
+        return unpack_fast_payload(host, self.fast["M"], self.params.num_joints)
+
+    def _result(self, st, host):
+        """Host payload of a blocking call -> per-image results of the pipeline's grouping mode."""
+        if self.grouping == "fast":
+            return self.unpack_fast(host)
+        return self.unpack(host, st["row"], st["T"], self.fetch_overflow(st, host))
 
     # -- device step (everything between the H2D copy and the D2H copy) -------------
     def _device_step(self, st, x):
@@ -274,6 +380,11 @@ class LitePosePipeline(object):
             main.wait_event(ov["P_done"][b])      # the parser that last read det/tag[b] has finished
         st["x"].copy_(x_dev, non_blocking=True)
         if ov["gF"][b] is None:
+            # the eager warm-up below writes the parser's buffers, which the other slot's parser graph (still running
+            # on the parser stream) shares
+            for ev in ov["P_done"]:
+                if ev is not None:
+                    main.wait_event(ev)
             self.engine.use_graphs = False
             o, f = self._network_part(st, st["x"], slot=b)       # warm-up: builds plans, sets attributes
             self._glue_part(st, o, f, ov["det"][b], ov["tag"][b])
@@ -316,14 +427,18 @@ class LitePosePipeline(object):
             Hd, Wd = det_hw if det_hw is not None else ((s_h, s_w) if self.project else (s_h // 2, s_w // 2))
             dev = self.device
             row = J * (3 + T)
+            width = self.keep * row + self.keep + 1
+            if self.grouping == "fast":            # every person (M <= 32) x J x (x, y, val, tag) | count | KM status
+                width = self.fast["M"] * J * 4 + 2
             st = {
                 "x": torch.empty((n, 3, s_h, s_w), dtype=dtype, device=dev),
                 "side": torch.cuda.Stream(device=dev, priority=self.prio_net),
                 "det": torch.empty((n, J, Hd, Wd), dtype=torch.float32, device=dev),
                 "tag": torch.empty((n, 1 if self.tag_shared else J, Hd, Wd, T), dtype=torch.float32, device=dev),
-                "packed": torch.zeros((n, self.keep * row + self.keep + 1), dtype=torch.float32, device=dev),
-                "host": torch.empty((n, self.keep * row + self.keep + 1), dtype=torch.float32).pin_memory(),
+                "packed": torch.zeros((n, width), dtype=torch.float32, device=dev),
+                "host": torch.empty((n, width), dtype=torch.float32).pin_memory(),
                 "row": row, "T": T, "graph": None, "plant": plant, "trans": None, "full": None, "ov": None,
+                "fast": self._fast_buffers(n, J) if self.grouping == "fast" else None,
             }
             if self._final is not None:
                 st["trans"] = torch.zeros((n, 6), dtype=torch.float64, device=dev)
@@ -344,7 +459,8 @@ class LitePosePipeline(object):
 
     def step_device(self, x_dev, plant=None):
         """Frames already resident on the device (NCHW fp16/fp32).  Returns the packed device result
-        [N, keep*J*(3+T) + keep + 1] (keypoints, scores, person count)."""
+        [N, keep*J*(3+T) + keep + 1] (keypoints, scores, person count); with grouping="fast" [N, M*J*4 + 2] (every
+        person's keypoints, person count, KM status: unpack_fast_payload)."""
         n, _, s_h, s_w = x_dev.shape
         st = self._get_state(n, s_h, s_w, x_dev.dtype, plant)
         ov = st.get("ov")
@@ -376,7 +492,7 @@ class LitePosePipeline(object):
         st = self._get_state(n, x.shape[2], x.shape[3], x.dtype, plant)
         st["host"].copy_(packed, non_blocking=True)
         torch.cuda.current_stream().synchronize()
-        return self.unpack(st["host"], st["row"], st["T"], self.fetch_overflow(st, st["host"]))
+        return self._result(st, st["host"])
 
     # -- multi-scale test (TEST.SCALE_FACTOR with several entries; reference valid.py:198-229) ----------------------------
     def step_device_multiscale(self, xs, plant=None):
@@ -436,7 +552,7 @@ class LitePosePipeline(object):
         st = self._get_state(x1.shape[0], x1.shape[2], x1.shape[3], x1.dtype, plant, det_hw=det_hw)
         st["host"].copy_(packed, non_blocking=True)
         torch.cuda.current_stream().synchronize()
-        return self.unpack(st["host"], st["row"], st["T"], self.fetch_overflow(st, st["host"]))
+        return self._result(st, st["host"])
 
     def infer_images(self, images, mean=(0.485, 0.456, 0.406), std=(0.229, 0.224, 0.225), half=True, plant=None):
         """The body of the reference's evaluation loop (valid.py:198-233) for a batch of equally sized uint8 images
@@ -477,7 +593,7 @@ class LitePosePipeline(object):
             self._last_state = st                 # det / tag of this call stay readable there until the next call
             st["host"].copy_(packed, non_blocking=True)
             torch.cuda.current_stream().synchronize()
-            return self.unpack(st["host"], st["row"], st["T"], self.fetch_overflow(st, st["host"]))
+            return self._result(st, st["host"])
         finally:
             if prev is None:
                 self.set_final_preds(None)
@@ -592,10 +708,25 @@ class LitePosePipeline(object):
                 for k, i in enumerate(g.images):
                     if plant[i] is not None:
                         plant[i].apply(det[k:k + 1], tag[k:k + 1])
-            if self.tag_shared:
+            if self.tag_shared and self.grouping == "fast":
+                tag_full[:, :1].copy_(tag)          # the peak finder reads the shared map as plane 0 of the image's block
+            elif self.tag_shared:
                 tag_full.copy_(tag.expand(-1, J, -1, -1, -1))
         # (4) once per batch: ragged parser, get_final_preds, payload, D2H
         hw = np.ascontiguousarray(mp.det_hw, np.int32)
+        if self.grouping == "fast":
+            M = self.fast["M"]
+            b = self._fast_buffers(n, J, lambda k, shape, dt: self._grow("fast_" + k, int(np.prod(shape)), dt).view(shape))
+            width = M * J * 4 + 2
+            packed = self._grow("packed", n * width, torch.float32).view(n, width)
+            self._fast_parse(b, det_a, tag_a, n, J, T, 1 if self.tag_shared else J, hw, d.data_ptr() + offs[-2],
+                             d.data_ptr() + offs[-1], packed)
+            out_h = self._grow("host", n * width, torch.float32, pinned=True).view(n, width)
+            out_h.copy_(packed, non_blocking=True)
+            main.synchronize()
+            res = self.unpack_fast(out_h)
+            self._last_mixed = {"plan": mp, "det": det_a, "tag": tag_a, "inputs": xs_arena}
+            return [res[int(p)] for p in mp.pos]
         ans, num, scores = self.parser.run_ragged(det_a, tag_a, hw, d[offs[-2]:].data_ptr(), T, self.adjust, self.refine)
         pcap = ans.shape[1]
         _lib.check(self.lib.lp_transform_preds_f32(ans.data_ptr(), num.data_ptr(), d.data_ptr() + offs[-1], n, pcap, J,
@@ -695,6 +826,9 @@ class LitePosePipeline(object):
         sl["busy"] = False
         if a["world"] > 1 and a["rank"] != a["dst"]:
             return None
+        if self.grouping == "fast":
+            res = [self.unpack_fast(sl["host"][r]) for r in range(sl["host"].shape[0])]      # raises on a KM status 1
+            return res if unpack else sl["host"]
         if float(sl["host"][:, :, -1].max()) > self.keep:
             raise _lib.LitePoseError("an image holds more persons than the packed payload carries (%d): use step() or "
                                      "a larger keep" % self.keep)

@@ -3,7 +3,8 @@ torch.profiler with CUDA activities: total device time, launches and share of th
 
 The step runs without CUDA graphs so that every launch is its own trace record; kernel times are those of the graphed
 step, the gaps between kernels are not.  As in the benchmark, the plain and the mirrored pass are two batch-N launch
-sequences on two streams.  Numbers printed under the profiler are a breakdown, not bench values."""
+sequences on two streams.  Numbers printed under the profiler are a breakdown, not bench values.  ``--demo`` takes the
+demo's settings (flip test, adjust and refine off), ``--grouping fast`` the pipeline's fast grouping mode."""
 import argparse
 import collections
 import os
@@ -44,15 +45,20 @@ def main():
     ap.add_argument("--people", type=int, default=5)
     ap.add_argument("--steps", type=int, default=5, help="profiled steps; totals are per step")
     ap.add_argument("--out", default=None, help="also write the table to this file")
+    ap.add_argument("--demo", action="store_true", help="the demo's settings: flip test, adjust and refine off")
+    ap.add_argument("--grouping", default="ae", choices=["ae", "fast"], help="the pipeline's grouping mode")
     a = ap.parse_args()
 
     dev = torch.device("cuda", 0)
-    cfg = get_cfg(input_size=a.size)
+    if a.demo:
+        cfg = get_cfg(input_size=a.size, flip_test=False, adjust=False, refine=False)
+    else:
+        cfg = get_cfg(input_size=a.size)
     torch.manual_seed(0)
     model = synth.scale_heads_(synth.randomize_bn_(get_pose_net(cfg, False, get_arch(a.arch)), 1)).eval().to(dev)
-    pipe = LitePosePipeline(model, cfg, use_graphs=False)
+    pipe = LitePosePipeline(model, cfg, use_graphs=False, grouping=a.grouping)
     x = synth.make_frames(a.batch, a.size, seed=1234).half().to(dev)
-    plant = PlantedCrowd(a.batch, 14, a.size, a.size, 2, num_people=a.people, seed=77, device=dev)
+    plant = PlantedCrowd(a.batch, 14, a.size, a.size, 2 if pipe.flip else 1, num_people=a.people, seed=77, device=dev)
     for _ in range(3):
         pipe.step_device(x, plant)
     torch.cuda.synchronize()
@@ -76,11 +82,13 @@ def main():
     kern_us = sum(tot.values()) / a.steps
     name, limit = gpu_info()
     lines = ["# %s, power limit %s" % (name, limit),
-             "# LitePose-%s %dx%d batch %d, one step = 2 backbone passes (flip) + glue + parser, no CUDA graphs, %d steps profiled"
-             % (a.arch, a.size, a.size, a.batch, a.steps),
+             "# LitePose-%s %dx%d batch %d, one step = %s + glue + %s parser, no CUDA graphs, %d steps profiled"
+             % (a.arch, a.size, a.size, a.batch, "2 backbone passes (flip)" if pipe.flip else "1 backbone pass",
+                a.grouping, a.steps),
              "# step wall time under the profiler %.3f ms; summed device time of all kernels/copies %.3f ms per step"
              % (step_ms, kern_us / 1e3),
-             "# the plain and the mirrored pass run concurrently on two streams, so summed device time exceeds wall time",
+             "# the plain and the mirrored pass run concurrently on two streams, so summed device time exceeds wall time"
+             if pipe.flip else "# summed device time exceeds wall time where kernels overlap",
              "# share = kernel time / summed device time",
              "%10s %8s %7s  %s" % ("us/step", "launches", "share", "kernel")]
     for k, v in sorted(tot.items(), key=lambda kv: -kv[1]):
