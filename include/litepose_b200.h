@@ -76,9 +76,9 @@ int lp_stem_conv3x3_s2(const void* x, int x_is_fp32, int flip_x, const void* w, 
 /* ---- M1 fused: the whole stem (conv3x3 s2 + BN + ReLU6 -> dw3x3 + BN + ReLU6 -> 1x1 + BN) in ONE kernel ----------
  * reference lib/models/pose_mobilenet.py:36-41.  x NCHW fp32/fp16 as above (flip_x = mirrored pass); w1_packed [32][64]
  * fp16: row co = the 27 BN-folded taps of output channel co (k = c*9 + ky*3 + kx), zero padded; w_dw [9][32] tap-major;
- * w_pw_packed / b_pw_packed from lp_pw1x1_pack(K = 32, N = C0); out [N,H/2,W/2,C0] fp16 NHWC (flip_x == 2: out [2N,...] -
- * the plain pass of the N images followed by their mirrored pass, the flip test as ONE batch).  The two 32-channel
- * half-resolution intermediates never reach HBM.  lp_stem_fused_supported: H even, W % 4 == 0, C0 % 8 == 0, C0 <= 32. */
+ * w_pw_packed / b_pw_packed from lp_pw1x1_pack(K = 32, N = C0); out [N,H/2,W/2,C0] fp16 NHWC.  flip_x must be 0 or 1
+ * (LP_ERR_BAD_ARG otherwise).  The two 32-channel half-resolution intermediates never reach HBM.
+ * lp_stem_fused_supported: H even, W % 4 == 0, C0 % 8 == 0, C0 <= 32. */
 int lp_stem_fused_supported(int H, int W, int C0);
 int lp_stem_fused_f16(const void* x, int x_is_fp32, int flip_x, const void* w1_packed, const float* b1, const void* w_dw,
                       const float* b_dw, const void* w_pw_packed, const float* b_pw_packed, void* out, int N, int H, int W,
@@ -91,7 +91,7 @@ int lp_dwconv_f16(const void* x, const void* w, const float* bias, void* y, int 
                   int W, int k, int stride, int act, lp_stream_t stream);
 /* Depthwise arithmetic of lp_dwconv_f16: 0 = every product accumulated in fp32, 1 = the k taps of one kernel
  * row accumulated in packed fp16 (HFMA2), row sums in fp32, 2 = fully packed fp16 (chains of two kernel rows folded
- * into a running fp16 total - the arithmetic of the fused block kernels).  Any other value (or env LP_DW_PREC unset)
+ * into a running fp16 total - the arithmetic of the fused block kernels).  Any other value (and the initial state)
  * selects the default: 2 for k = 7 and k = 3 (backbone, stem), 0 for k = 5 (heads).  Process-wide; set before
  * building engines / capturing graphs. */
 void lp_set_dw_precision(int prec);

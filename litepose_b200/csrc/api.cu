@@ -2,7 +2,6 @@
 // tensor-map construction through the driver entry point (no link-time libcuda dependency).
 #include <atomic>
 #include <cstdarg>
-#include <cstdlib>
 #include <cstring>
 #include <mutex>
 
@@ -96,15 +95,6 @@ int make_tmap(CUtensorMap* map, const void* base, int rank, const uint64_t* dims
     return LP_OK;
 }
 
-bool pdl_enabled() {
-    static int v = -1;
-    if (v < 0) {
-        const char* e = getenv("LP_PDL");
-        v = (e && e[0] == '0') ? 0 : 1;
-    }
-    return v != 0;
-}
-
 int num_sms() {
     static thread_local int cached_dev = -1;
     static thread_local int cached = 0;
@@ -115,13 +105,6 @@ int num_sms() {
         if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;
         cached = v;
         cached_dev = dev;
-    }
-    // experiment knob: persistent kernels size their grids with fewer SMs (e.g. half the chip per pass of the flip test,
-    // so that the plain and the mirrored pass run side by side instead of alternating whole-chip kernels)
-    const char* e = getenv("LP_GRID_SMS");
-    if (e && e[0]) {
-        const int v = atoi(e);
-        if (v > 0 && v < cached) return v;
     }
     return cached;
 }

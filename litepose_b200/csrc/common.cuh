@@ -49,8 +49,7 @@ int num_sms();
 
 // Programmatic dependent launch (PDL): kernels launched through launch_pdl() may start their prologue (barrier init,
 // descriptor prefetch, weight staging) while the previous kernel of the stream drains; they call
-// pdl_wait() before touching any activation memory.  LP_PDL=0 in the environment disables the launch attribute.
-bool pdl_enabled();
+// pdl_wait() before touching any activation memory.
 
 #ifdef __CUDACC__
 template <typename... KArgs, typename... Args>
@@ -66,7 +65,7 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled() ? 1 : 0;
+    cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 #endif

@@ -334,14 +334,7 @@ void deconv_rows_pack(const uint16_t* wr, const uint16_t* ww, int Cr, int Cw, in
     dr_pack(Cr, Cw, Co, wr, ww, wp);
 }
 // the row kernel pays off on wide maps (a strip is 128 pixels); narrow levels keep the tiled kernel
-bool deconv_rows_shape_ok(int W) {
-    static int mode = -1;
-    if (mode < 0) {
-        const char* e = getenv("LP_DECONV_ROWS");
-        mode = (e && e[0] == '0') ? 0 : 1;
-    }
-    return mode != 0 && W >= 64;
-}
+bool deconv_rows_shape_ok(int W) { return W >= 64; }
 
 int launch_deconv_rows(const void* refined, const void* raw, const void* w_rows, const float* bias_packed, void* out, int N,
                        int H, int W, int Cr, int Cw, int Co, cudaStream_t stream) {

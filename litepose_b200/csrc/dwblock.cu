@@ -16,8 +16,6 @@
 //     global/L2), fp16 stores.
 // Warp roles: 0-15 depthwise + MMA (two groups of 8 = even / odd 32-channel slabs), 16 TMA producer.
 // HBM traffic of a block: read N*H*W*Cin*2 (x1.9 halo, L2 hits) + identity row, write N*H*W*Co*2.
-#include <stdlib.h>
-
 #include "common.cuh"
 #include "dw_inner.cuh"
 
@@ -61,7 +59,6 @@ struct BkParams {
     int nslabs, nkb, k16;             // k16 = K=16 MMA steps that carry input channels (ceil(Cin/16))
     int off_we, off_slab, off_dww, off_a, off_wp, off_bias;   // shared-memory layout (bytes)
     int wp_stage;                     // streaming mode: bytes of one projection-weight ring slot
-    int skew_ns;                      // group 1 starts every tile this much later (phase offset of the two groups)
     const float* b_exp;               // [Ce]
     const float* b_dw;                // [Ce]
     const float* b_pj;                // packed, n_tile
@@ -201,7 +198,6 @@ block_s1_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
         pdl_wait();                                        // the identity rows are read from global memory
         for (int t = blockIdx.x; t < p.num_tiles; t += gridDim.x, ++it) {
             const int tx = t % p.tiles_x, ty = (t / p.tiles_x) % p.tiles_y, n = t / (p.tiles_x * p.tiles_y);
-            if (grp && p.skew_ns) __nanosleep(p.skew_ns);
             // Odd slab counts (Ce = 96: 3 slabs) leave one group idle in the last round of a tile; the groups therefore swap
             // roles on odd tiles (group 0 takes the odd slabs), so that over two tiles each group runs the same number of
             // slabs.
@@ -434,14 +430,6 @@ extern "C" int lp_block_s1_f16(const void* x, const void* w_exp_packed, const fl
     p.b_dw = b_dw;
     p.b_pj = b_proj_packed;
     p.residual = identity ? reinterpret_cast<const __half*>(x) : nullptr;
-    {
-        static int skew = -1;
-        if (skew < 0) {
-            const char* e = getenv("LP_BLOCK_SKEW_NS");
-            skew = e ? atoi(e) : 0;
-        }
-        p.skew_ns = skew;
-    }
     p.out = reinterpret_cast<__half*>(out);
     CUtensorMap mx, mwe, mdw, mwp;
     {

@@ -9,8 +9,6 @@
 // compute loop has no boundary branches.  Each thread owns one channel PAIR (half2) and walks
 // 4x4 output micro-blocks with the k*k half2 weights held in registers, accumulating in fp32.
 // Algorithmic bytes per launch: 2*(N*C*Hin*Win + N*C*Hout*Wout + C*k*k) (+4*C bias).
-#include <cstdlib>
-
 #include "common.cuh"
 
 namespace lp {
@@ -186,14 +184,10 @@ dwconv_kernel(const __grid_constant__ CUtensorMap map_x, const __half* __restric
 }
 
 // Depthwise arithmetic of this (unfused) kernel: 0 = fp32 accumulation, 1 = packed fp16 row sums added in fp32,
-// 2 = fully packed fp16 (grouped chains, like the fused block kernels).  Default (LP_DW_PREC unset): 2 for the
-// backbone / stem kernels k = 7 and k = 3, 0 for k = 5 (the SepConv heads feed the network outputs directly).
-static int g_dw_prec = -1;   // -1: read LP_DW_PREC once; -2: per-kernel-size default
+// 2 = fully packed fp16 (grouped chains, like the fused block kernels).  Default: 2 for the backbone / stem kernels
+// k = 7 and k = 3, 0 for k = 5 (the SepConv heads feed the network outputs directly).
+static int g_dw_prec = -2;   // -2: per-kernel-size default
 static int dw_prec(int k) {
-    if (g_dw_prec == -1) {
-        const char* e = getenv("LP_DW_PREC");
-        g_dw_prec = (e && e[0] >= '0' && e[0] <= '2') ? e[0] - '0' : -2;
-    }
     if (g_dw_prec == -2) return k == 5 ? 0 : 2;
     return g_dw_prec;
 }

@@ -13,8 +13,6 @@
 //                rounds), including its `abs(t) < 1e-2` which binds to int abs(int) with its includes: trunc(t) == 0.
 // The reference's [10] stack arrays (assign.cpp:46-48,79-80) are lifted to 32 entries; its unbounded KM loop is capped
 // (status 1 is reported where the reference would not return).
-#include <stdlib.h>
-
 #include "common.cuh"
 
 namespace lp {
@@ -201,7 +199,7 @@ __device__ bool fu_match(const FuShared& s, FuKm& k, int n, int u0, int lane) {
 }
 
 // assign.cpp:45-66; false when the round cap is hit (the reference has none)
-__device__ bool fu_km(FuShared& s, int n, int lane, bool ff) {
+__device__ bool fu_km(FuShared& s, int n, int lane) {
     FuKm k;
     k.Lx = -1e6f;
     if (lane < n)
@@ -237,7 +235,7 @@ __device__ bool fu_km(FuShared& s, int n, int lane, bool ff) {
             //     columns is ever consumed), a status flip ends the walk before that round is skipped;
             //   * pairs with an unvisited column drop by at most d + DELTA per round: a conservative bound on the number of
             //     rounds for which they stay non-tight and >= d is computed once.
-            const bool walk = ff && (k.S == prevS) && (k.T == prevT) && d > 0.f;
+            const bool walk = (k.S == prevS) && (k.T == prevT) && d > 0.f;
             prevS = k.S;
             prevT = k.T;
             if (walk) {
@@ -329,7 +327,7 @@ __device__ bool fu_km(FuShared& s, int n, int lane, bool ff) {
 __global__ void __launch_bounds__(32)
 assign_kernel(const int* __restrict__ count, const float* __restrict__ val, const float* __restrict__ tag,
               const int* __restrict__ ind, const int* __restrict__ joint_order, int C, int M, float threshold,
-              int* __restrict__ num_person, float* __restrict__ ans, int* __restrict__ status, int ff) {
+              int* __restrict__ num_person, float* __restrict__ ans, int* __restrict__ status) {
     __shared__ FuShared s;
     const int img = blockIdx.x, lane = threadIdx.x;
     const int* cnt = count + (size_t)img * C;
@@ -374,7 +372,7 @@ assign_kernel(const int* __restrict__ count, const float* __restrict__ val, cons
             }
         }
         __syncwarp();
-        if (!fu_km(s, n, lane, ff != 0)) {
+        if (!fu_km(s, n, lane)) {
             st = 1;
             break;
         }
@@ -461,13 +459,8 @@ extern "C" int lp_assign_f32(const int* count, const float* val, const float* ta
         set_error("lp_assign_f32: max_count %d exceeds the %d candidates/persons this build holds per joint", M, FU_MAXP);
         return LP_ERR_CAPACITY;
     }
-    static int ff = -1;
-    if (ff < 0) {
-        const char* e = getenv("LP_FU_FASTFORWARD");     // ablation switch; default on
-        ff = (e && e[0] == '0') ? 0 : 1;
-    }
     assign_kernel<<<N, 32, 0, (cudaStream_t)stream>>>(count, val, tag, ind, joint_order, C, M, threshold, num_person, ans,
-                                                     status, ff);
+                                                     status);
     LP_LAUNCH_CHECK("assign_kernel");
     return LP_OK;
 }

@@ -43,7 +43,7 @@ constexpr int SF_T = 4 * SF_TCHUNK;
 struct SfParams {
     int N, H, W, Ho, Wo, C0, n_tile;
     int tiles_x, tiles_y, num_tiles;
-    int flip_x, x_is_fp32;    // flip_x: 0 plain, 1 mirrored, 2 pair batch (images N/2.. are the mirrored copies of 0..N/2-1)
+    int flip_x, x_is_fp32;    // flip_x: 0 plain, 1 mirrored
     const void* x;
     const float* b1;        // [32]
     const __half* w_dw;     // [9][32] tap-major
@@ -74,11 +74,8 @@ __device__ __forceinline__ uint4 sf_load_vec(const SfParams& p, int t, int i) {
     const int gy = 2 * ty * SF_TH - 3 + r, gx = 2 * tx * SF_TW - 4 + 4 * v;
     uint4 o = make_uint4(0u, 0u, 0u, 0u);
     if (gy >= 0 && gy < p.H && gx >= 0 && gx < p.W) {       // gx % 4 == 0 and W % 4 == 0: all four or none inside
-        const int half = p.N >> 1;
-        const bool fl = p.flip_x == 2 ? n >= half : p.flip_x != 0;
-        const int ns = (p.flip_x == 2 && n >= half) ? n - half : n;
-        const int sx = fl ? p.W - 4 - gx : gx;
-        const size_t off = (((size_t)ns * 3 + c) * p.H + gy) * p.W + sx;
+        const int sx = p.flip_x ? p.W - 4 - gx : gx;
+        const size_t off = (((size_t)n * 3 + c) * p.H + gy) * p.W + sx;
         if (FP32) {
             o = __ldg(reinterpret_cast<const uint4*>(reinterpret_cast<const float*>(p.x) + off));
         } else {
@@ -158,7 +155,7 @@ stem_fused_kernel(const __grid_constant__ CUtensorMap map_w1, const __grid_const
             if (i < SF_NV) {
                 const int v = i % SF_PV, rr = i / SF_PV;
                 *reinterpret_cast<uint2*>(&sm.patch[rr / SF_PH][rr % SF_PH][4 * v]) =
-                    sf_pack_vec<FP32>(pre[u], p.flip_x == 2 ? (n >= (p.N >> 1)) : p.flip_x);
+                    sf_pack_vec<FP32>(pre[u], p.flip_x);
             }
         }
         __syncthreads();
@@ -312,6 +309,7 @@ extern "C" int lp_stem_fused_f16(const void* x, int x_is_fp32, int flip_x, const
     LP_CHECK_ARG(N > 0 && lp_stem_fused_supported(H, W, C0),
                  "lp_stem_fused_f16: unsupported shape N=%d H=%d W=%d C0=%d (H even, W %% 4 == 0, C0 %% 8 == 0, C0 <= 32)", N,
                  H, W, C0);
+    LP_CHECK_ARG(flip_x == 0 || flip_x == 1, "lp_stem_fused_f16: flip_x=%d (0 plain, 1 mirrored)", flip_x);
     if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(w1_packed) |
          reinterpret_cast<uintptr_t>(w_pw_packed)) & 15) {
         set_error("lp_stem_fused_f16: pointers must be 16-byte aligned");
@@ -319,7 +317,6 @@ extern "C" int lp_stem_fused_f16(const void* x, int x_is_fp32, int flip_x, const
     }
     SfParams p;
     memset(&p, 0, sizeof(p));
-    if (flip_x == 2) N *= 2;          // pair batch: N input images -> 2N outputs (plain pass, then the mirrored pass)
     p.N = N; p.H = H; p.W = W; p.Ho = H / 2; p.Wo = W / 2; p.C0 = C0;
     p.n_tile = (C0 + 15) / 16 * 16;
     p.tiles_x = (p.Wo + SF_TW - 1) / SF_TW;

@@ -85,11 +85,6 @@ class LitePoseEngine(object):
         self.arena_plans = collections.OrderedDict()    # LRU of plans whose buffers live in self.arenas
         self.arenas = {}                                # pass -> uint8 arena shared by every arena plan of that pass
         self.use_graphs = False
-        import os
-        self.fuse_dw_project = os.environ.get("LP_FUSE_DW_PROJECT", "1") != "0"
-        self.fuse_heads = os.environ.get("LP_FUSE_HEADS", "1") != "0"
-        self.fuse_block = os.environ.get("LP_FUSE_BLOCK", "1") != "0"
-        self.fuse_stem = os.environ.get("LP_FUSE_STEM", "1") != "0"
 
     # ------------------------------------------------------------------ folded checkpoint ("next" row 4)
     # BN fold (reference fuse_bn.py:81-162) and kernel packing become a load-time no-op: the file holds exactly the
@@ -250,11 +245,8 @@ class LitePoseEngine(object):
                 w1 = sd["final_refined.%d.conv.3.weight" % (i - 1)].float()
                 w2 = sd["final_raw.%d.conv.3.weight" % (i - 1)].float()
                 co, c1, c2 = w1.shape[0], w1.shape[1], w2.shape[1]
-                wp = np.zeros(self.lib.lp_head_packed_elems(c1, c2, co), np.uint16)
                 a, c = _np16(w1.reshape(co, c1)), _np16(w2.reshape(co, c2))
-                _lib.check(self.lib.lp_head_pack(a.ctypes.data, c.ctypes.data, c1, c2, co, wp.ctypes.data),
-                           "lp_head_pack")
-                hd.update({"w": self._dev(wp, torch.float16), "C1": c1, "C2": c2, "Co": co})
+                hd.update({"C1": c1, "C2": c2, "Co": co})
                 # fused head: concatenated depthwise slabs + slab-ordered 1x1 weights
                 d1, d2 = hd["final_refined_dw"], hd["final_raw_dw"]
                 dwc = np.zeros(self.lib.lp_head_fused_dw_elems(c1, c2), np.uint16)
@@ -272,9 +264,8 @@ class LitePoseEngine(object):
         self.P = P
 
     # ------------------------------------------------------------------ plan
-    def _build_plan(self, n, h, w, in_dtype, out_fp32, pair=False, alloc=None):
-        """pair: the flip test as ONE batch of 2n (images n.. are the mirrored copies, produced by the fused stem).
-        alloc(shape, dtype) provides every buffer of the plan (default: a tensor of its own)."""
+    def _build_plan(self, n, h, w, in_dtype, out_fp32, alloc=None):
+        """alloc(shape, dtype) provides every buffer of the plan (default: a tensor of its own)."""
         if h % 16 or w % 16:
             raise ValueError("LitePose input height/width must be multiples of 16, got %dx%d" % (h, w))
         lib, P, dev = self.lib, self.P, self.device
@@ -288,21 +279,16 @@ class LitePoseEngine(object):
             return alloc(shape, f16)
 
         plan = {"in_ptr": ctypes.c_void_p(0), "flip": ctypes.c_int(0)}
-        n_in = n
-        if pair:
-            if not (self.fuse_stem and lib.lp_stem_fused_supported(h, w, P["stem_pw"]["N"])):
-                raise ValueError("pair-batch mode needs the fused stem (H even, W % 4 == 0)")
-            n = 2 * n
         h2, w2 = h // 2, w // 2
         x0 = buf(n, h2, w2, P["stem_pw"]["N"])
         st, d, q = P["stem"], P["stem_dw"], P["stem_pw"]
         keep = [x0]
-        if self.fuse_stem and "w1p" in st and lib.lp_stem_fused_supported(h, w, q["N"]):
+        if "w1p" in st and lib.lp_stem_fused_supported(h, w, q["N"]):
             # conv3x3 s2 -> dw3x3 -> 1x1 in one kernel: the two 32-channel half-resolution tensors never reach HBM
             ops.append(_Op("stem_fused", lib.lp_stem_fused_f16,
                            [plan["in_ptr"], 1 if in_dtype == torch.float32 else 0, plan["flip"], st["w1p"].data_ptr(),
                             st["b"].data_ptr(), d["w"].data_ptr(), d["b"].data_ptr(), q["w"].data_ptr(), q["b"].data_ptr(),
-                            x0.data_ptr(), n_in, h, w, q["N"]]))
+                            x0.data_ptr(), n, h, w, q["N"]]))
         else:
             a0 = buf(n, h2, w2, 32)
             a1 = buf(n, h2, w2, 32)
@@ -333,7 +319,7 @@ class LitePoseEngine(object):
             oh, ow = ch // blk["stride"], cw_ // blk["stride"]
             out = buf(n, oh, ow, pc["N"])
             keep.append(out)
-            if self.fuse_block and self.fuse_dw_project and "wblk" in inv:
+            if "wblk" in inv:
                 # the whole block in one kernel: the 6x-expanded tensor never reaches HBM
                 ops.append(_Op("block_s1", lib.lp_block_s1_f16,
                                [cur.data_ptr(), inv["wblk"].data_ptr(), inv["bblk"].data_ptr(), dw["w"].data_ptr(),
@@ -346,7 +332,7 @@ class LitePoseEngine(object):
             ops.append(_Op("inv", lib.lp_pw1x1_f16, [cur.data_ptr(), inv["w"].data_ptr(), inv["b"].data_ptr(), None,
                                                       e_buf.data_ptr(), n * ch * cw_, inv["K"], inv["N"],
                                                       _lib.ACT_RELU6]))
-            if self.fuse_dw_project and blk["stride"] == 1 and dw["k"] == 7 and pc["N"] <= 160 and dw["C"] <= 992:
+            if blk["stride"] == 1 and dw["k"] == 7 and pc["N"] <= 160 and dw["C"] <= 992:
                 # depthwise + projection (+ identity) in one kernel: the expanded dw output never reaches HBM
                 ops.append(_Op("dw7_project", lib.lp_dw7_project_f16,
                                [e_buf.data_ptr(), dw["w"].data_ptr(), dw["b"].data_ptr(), pc["w"].data_ptr(),
@@ -378,22 +364,10 @@ class LitePoseEngine(object):
                 hd = P["heads"][i - 1]
                 o = alloc((n, hd["Co"], rh, rw), torch.float32 if out_fp32 else f16)
                 outs.append(o)
-                if self.fuse_heads:
-                    ops.append(_Op("head_fused", lib.lp_head_fused_f16,
-                                   [refined.data_ptr(), raw.data_ptr(), hd["dw_cat"].data_ptr(),
-                                    hd["bdw_cat"].data_ptr(), hd["pw_cat"].data_ptr(), o.data_ptr(),
-                                    1 if out_fp32 else 0, n, rh, rw, hd["C1"], hd["C2"], hd["Co"]]))
-                else:
-                    t1, t2 = buf(n, rh, rw, hd["C1"]), buf(n, rh, rw, hd["C2"])
-                    keep += [t1, t2]
-                    for src, dst, key in ((refined, t1, "final_refined_dw"), (raw, t2, "final_raw_dw")):
-                        dd = hd[key]
-                        ops.append(_Op("head_dw", lib.lp_dwconv_f16,
-                                       [src.data_ptr(), dd["w"].data_ptr(), dd["b"].data_ptr(), dst.data_ptr(), n,
-                                        dd["C"], rh, rw, dd["k"], 1, _lib.ACT_RELU]))
-                    ops.append(_Op("head_pw", lib.lp_head_pw_dual_f16,
-                                   [t1.data_ptr(), t2.data_ptr(), hd["w"].data_ptr(), o.data_ptr(),
-                                    1 if out_fp32 else 0, n, rh, rw, hd["C1"], hd["C2"], hd["Co"]]))
+                ops.append(_Op("head_fused", lib.lp_head_fused_f16,
+                               [refined.data_ptr(), raw.data_ptr(), hd["dw_cat"].data_ptr(),
+                                hd["bdw_cat"].data_ptr(), hd["pw_cat"].data_ptr(), o.data_ptr(),
+                                1 if out_fp32 else 0, n, rh, rw, hd["C1"], hd["C2"], hd["Co"]]))
         plan.update({"ops": ops, "outs": outs, "keep": keep, "graph": None, "static_in": None})
         return plan
 
@@ -401,16 +375,12 @@ class LitePoseEngine(object):
         # the flip pass owns its own buffers so that both passes can be in flight at once; ``slot`` selects one of
         # several buffer sets (the pipeline alternates two so that step i+1's passes never touch the outputs step i's
         # glue is still reading)
-        key = (n, h, w, in_dtype, out_fp32, flip if flip == "both" else bool(flip), slot)
+        key = (n, h, w, in_dtype, out_fp32, bool(flip), slot)
         pl = self.plans.get(key)
         if pl is None:
-            pl = self._build_plan(n, h, w, in_dtype, out_fp32, pair=(flip == "both"))
+            pl = self._build_plan(n, h, w, in_dtype, out_fp32)
             self.plans[key] = pl
         return pl
-
-    @staticmethod
-    def _pass_of(flip):
-        return flip if flip == "both" else bool(flip)
 
     def reserve_arena(self, specs):
         """Size the arenas for the plans ``specs`` = [(n, h, w, in_dtype, out_fp32, flip)] before any of them runs.
@@ -419,8 +389,8 @@ class LitePoseEngine(object):
         need = {}
         for n, h, w, in_dtype, out_fp32, flip in specs:
             m = _Bump()
-            self._build_plan(n, h, w, in_dtype, out_fp32, pair=(flip == "both"), alloc=m)
-            key = self._pass_of(flip)
+            self._build_plan(n, h, w, in_dtype, out_fp32, alloc=m)
+            key = bool(flip)
             need[key] = max(need.get(key, 0), m.used)
         for key, nbytes in need.items():
             ar = self.arenas.get(key)
@@ -434,13 +404,13 @@ class LitePoseEngine(object):
         """A plan whose buffers are carved out of the arena of its pass (plain / mirrored): plans of every size share
         that memory, so device memory does not grow with the number of distinct (n, h, w) served.  Arena plans of one
         pass must run in stream order (the pipeline's mixed batches do); at most ARENA_PLANS are kept."""
-        key = (n, h, w, in_dtype, out_fp32, self._pass_of(flip))
+        key = (n, h, w, in_dtype, out_fp32, bool(flip))
         pl = self.arena_plans.get(key)
         if pl is not None:
             self.arena_plans.move_to_end(key)
             return pl
         self.reserve_arena([(n, h, w, in_dtype, out_fp32, flip)])
-        pl = self._build_plan(n, h, w, in_dtype, out_fp32, pair=(flip == "both"), alloc=_Bump(self.arenas[key[5]]))
+        pl = self._build_plan(n, h, w, in_dtype, out_fp32, alloc=_Bump(self.arenas[key[5]]))
         self.arena_plans[key] = pl
         while len(self.arena_plans) > ARENA_PLANS:
             self.arena_plans.popitem(last=False)
@@ -455,9 +425,8 @@ class LitePoseEngine(object):
 
     def run(self, x, flip=False, out_fp32=True, clone=True, slot=0, arena=False):
         """x: NCHW fp16/fp32 CUDA tensor.  Returns [out0 [N,2J,H/4,W/4], out1 [N,J,H/2,W/2]]
-        (fp32 when out_fp32 else fp16).  ``flip`` computes the forward of torch.flip(x,[3]); ``flip="both"`` runs the flip test
-        as ONE batch of 2N (outputs [2N, ...]: rows N.. belong to the mirrored images).  ``arena``: run on an arena plan
-        (arena_plan_for; eager launches only) - its outputs are overwritten by the next arena run of the same pass."""
+        (fp32 when out_fp32 else fp16).  ``flip`` computes the forward of torch.flip(x,[3]).  ``arena``: run on an arena
+        plan (arena_plan_for; eager launches only) - its outputs are overwritten by the next arena run of the same pass."""
         if self.device.type != "cuda":
             raise RuntimeError("LitePoseEngine.run needs a CUDA device (this engine was prepared on %s)" % self.device)
         assert x.is_cuda and x.dim() == 4 and x.shape[1] == 3
@@ -481,7 +450,7 @@ class LitePoseEngine(object):
                 plan["static_in"].copy_(x)
                 if key not in g:
                     plan["in_ptr"].value = plan["static_in"].data_ptr()
-                    plan["flip"].value = 2 if flip == "both" else (1 if flip else 0)
+                    plan["flip"].value = 1 if flip else 0
                     self._launch_all(plan, stream)      # warm-up (also sets func attributes)
                     torch.cuda.current_stream().synchronize()
                     cg = torch.cuda.CUDAGraph()
@@ -491,7 +460,7 @@ class LitePoseEngine(object):
                 g[key].replay()
             else:
                 plan["in_ptr"].value = x.data_ptr()
-                plan["flip"].value = 2 if flip == "both" else (1 if flip else 0)
+                plan["flip"].value = 1 if flip else 0
                 self._launch_all(plan, stream)
         outs = plan["outs"]
         return [o.clone() for o in outs] if clone else list(outs)

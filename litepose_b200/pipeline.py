@@ -142,13 +142,6 @@ class LitePosePipeline(object):
         self.tag_shared = not bool(cfg.MODEL.TAG_PER_JOINT)
         self.canonical = self.model_joints == p.num_joints and not self.tag_shared
         self.use_graphs = use_graphs
-        import os
-        self.two_streams = os.environ.get("LP_TWO_STREAMS", "1") != "0"
-        self.pair_batch = os.environ.get("LP_PAIR_BATCH", "0") == "1"      # experiment: both passes as one batch of 2N
-        # experiment: CUDA stream priorities of the kernels captured into the network graph / the glue+parser graph of
-        # the overlapped step (0 = default; negative = higher priority)
-        self.prio_net = int(os.environ.get("LP_PRIO_NET", "0"))
-        self.prio_parser = int(os.environ.get("LP_PRIO_PARSER", "0"))
         # persons per image in the fixed-size packed payload (the D2H copy / NCCL gather of every step).  The reference
         # returns every person it finds (lib/core/group.py:96,269-291); an image with more than ``keep`` persons is
         # never clipped: step() fetches the full result from the parser's buffers (capacity J*K persons) in a second
@@ -232,27 +225,17 @@ class LitePosePipeline(object):
         """Both network passes -> ([o0, o1], [f0, f1]) in the engine's buffer set ``slot`` (``arena``: in the engine's
         shared arena plans, see LitePoseEngine.arena_plan_for)."""
         eng = self.engine
-        f = None
-        if self.flip and self.pair_batch:
-            # the flip test as ONE batch of 2N: half the launches, twice the tiles per persistent kernel
-            both = eng.run(x, flip="both", out_fp32=True, clone=False, slot=slot, arena=arena)
-            nb = x.shape[0]
-            o = [both[0][:nb], both[1][:nb]]
-            f = [both[0][nb:], both[1][nb:]]
-        elif self.flip and self.two_streams:
-            # the plain and the mirrored pass are independent until the glue: fork onto a side stream so that one pass'
-            # kernels fill the launch gaps and tails of the other (each pass has its own plan buffers)
-            main = torch.cuda.current_stream()
-            side = st["side"]
-            side.wait_stream(main)
-            with torch.cuda.stream(side):
-                f = eng.run(x, flip=True, out_fp32=True, clone=False, slot=slot, arena=arena)
-            o = eng.run(x, flip=False, out_fp32=True, clone=False, slot=slot, arena=arena)
-            main.wait_stream(side)
-        else:
-            o = eng.run(x, flip=False, out_fp32=True, clone=False, slot=slot, arena=arena)
-            if self.flip:
-                f = eng.run(x, flip=True, out_fp32=True, clone=False, slot=slot, arena=arena)
+        if not self.flip:
+            return eng.run(x, flip=False, out_fp32=True, clone=False, slot=slot, arena=arena), None
+        # the plain and the mirrored pass are independent until the glue: fork onto a side stream so that one pass'
+        # kernels fill the launch gaps and tails of the other (each pass has its own plan buffers)
+        main = torch.cuda.current_stream()
+        side = st["side"]
+        side.wait_stream(main)
+        with torch.cuda.stream(side):
+            f = eng.run(x, flip=True, out_fp32=True, clone=False, slot=slot, arena=arena)
+        o = eng.run(x, flip=False, out_fp32=True, clone=False, slot=slot, arena=arena)
+        main.wait_stream(side)
         return o, f
 
     def _glue_part(self, st, o, f, det, tag):
@@ -367,10 +350,7 @@ class LitePosePipeline(object):
         if ov is None:
             ov = st["ov"] = {"det": [st["det"], torch.empty_like(st["det"])], "tag": [st["tag"], torch.empty_like(st["tag"])],
                              "packed": [st["packed"], torch.zeros_like(st["packed"])], "gF": [None, None], "gP": [None, None],
-                             "pstream": torch.cuda.Stream(device=self.device, priority=self.prio_parser),
-                             "cap_net": torch.cuda.Stream(device=self.device, priority=self.prio_net),
-                             "cap_par": torch.cuda.Stream(device=self.device, priority=self.prio_parser),
-                             "P_done": [None, None],
+                             "pstream": torch.cuda.Stream(device=self.device), "P_done": [None, None],
                              "consumer_done": [None, None], "idx": 0}
         b = ov["idx"]
         ov["idx"] = b ^ 1
@@ -391,11 +371,11 @@ class LitePosePipeline(object):
             self._parser_part(st, ov["det"][b], ov["tag"][b], ov["packed"][b])
             torch.cuda.synchronize()
             g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g, stream=ov["cap_net"]):       # kernel nodes keep the capture stream's priority
+            with torch.cuda.graph(g):
                 o, f = self._network_part(st, st["x"], slot=b)
             ov["gF"][b] = g
             g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g, stream=ov["cap_par"]):
+            with torch.cuda.graph(g):
                 # the glue writes 1.4 GB at the HBM write roofline: on the second stream it overlaps the FMA-bound network
                 # passes of the next step (which write the other buffer set of the engine)
                 self._glue_part(st, o, f, ov["det"][b], ov["tag"][b])
@@ -432,7 +412,7 @@ class LitePosePipeline(object):
                 width = self.fast["M"] * J * 4 + 2
             st = {
                 "x": torch.empty((n, 3, s_h, s_w), dtype=dtype, device=dev),
-                "side": torch.cuda.Stream(device=dev, priority=self.prio_net),
+                "side": torch.cuda.Stream(device=dev),
                 "det": torch.empty((n, J, Hd, Wd), dtype=torch.float32, device=dev),
                 "tag": torch.empty((n, 1 if self.tag_shared else J, Hd, Wd, T), dtype=torch.float32, device=dev),
                 "packed": torch.zeros((n, width), dtype=torch.float32, device=dev),
@@ -633,7 +613,7 @@ class LitePosePipeline(object):
         mp = MixedPlan(shapes, self.scales, int(self.cfg.DATASET.INPUT_SIZE), self.project, J, T)
         if not hasattr(self, "_mixed_bufs"):
             self._mixed_bufs = {}
-            self._mixed_side = torch.cuda.Stream(device=self.device, priority=self.prio_net)
+            self._mixed_side = torch.cuda.Stream(device=self.device)
         dev = self.device
         in_dtype = torch.float16 if half else torch.float32
         main = torch.cuda.current_stream()
@@ -682,12 +662,9 @@ class LitePosePipeline(object):
         for g in mp.groups:
             for s in self.scales:
                 hs, ws = g.in_hw[s]
-                if self.flip and self.pair_batch:
-                    specs.append((g.n, hs, ws, in_dtype, True, "both"))
-                else:
-                    specs.append((g.n, hs, ws, in_dtype, True, False))
-                    if self.flip:
-                        specs.append((g.n, hs, ws, in_dtype, True, True))
+                specs.append((g.n, hs, ws, in_dtype, True, False))
+                if self.flip:
+                    specs.append((g.n, hs, ws, in_dtype, True, True))
         self.engine.reserve_arena(specs)
         st = {"side": self._mixed_side, "plant": None}
         for g in mp.groups:

@@ -260,19 +260,3 @@ def test_dataparallel_two_devices():
         ref = model(x)
     for a, b, old in zip(ref, again, multi):
         assert torch.equal(a, b) and not torch.equal(b, old)
-
-
-def test_pair_batch_equals_two_passes():
-    """engine.run(flip="both"): the flip test as one batch of 2N (the fused stem mirrors the second half) is bit-identical
-    to the plain pass + the mirrored pass"""
-    cfg = get_cfg(input_size=128)
-    torch.manual_seed(0)
-    model = synth.randomize_bn_(get_pose_net(cfg, False, get_arch("S")), 1).cuda().eval()
-    x = synth.make_frames(3, 128, seed=5).cuda().half()
-    eng = model.lp_engine()
-    a = eng.run(x, flip=False)
-    b = eng.run(x, flip=True)
-    both = eng.run(x, flip="both")
-    for i in range(2):
-        assert both[i].shape[0] == 6
-        assert torch.equal(both[i][:3], a[i]) and torch.equal(both[i][3:], b[i])

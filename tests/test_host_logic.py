@@ -76,6 +76,11 @@ def test_round2_entry_points_validate_arguments():
                                 None) == 1
     assert b"K<=64" in lib.lp_last_error()
     assert lib.lp_tag_match_workspace_bytes(2, 14, 64, 2, 14 * 64) == 2 * 14 * 64 * (4 + 4 + 14 * 2 * 4)
+    # flip_x is 0 (plain) or 1 (mirrored); anything else is refused, not read as "mirrored".  x is misaligned so that a
+    # library that accepted the flag would stop at its alignment check (LP_ERR_ALIGN) instead of launching
+    assert lib.lp_stem_fused_f16(ctypes.c_void_p(8), 0, 2, one, None, one, None, one, None, one, 2, 16, 16, 16,
+                                 None) == 1
+    assert b"flip_x" in lib.lp_last_error()
 
 
 def test_pipeline_cfg_validation_is_host_side():

@@ -64,4 +64,4 @@ try:
     gpu = r.stdout.strip().splitlines()[0]
 except Exception:
     gpu = torch.cuda.get_device_name(0)
-print(json.dumps({"gpu": gpu, "skew_ns": os.environ.get("LP_BLOCK_SKEW_NS", "0"), "shapes": out}))
+print(json.dumps({"gpu": gpu, "shapes": out}))
