@@ -131,6 +131,16 @@ int lp_block_s1_f16(const void* x, const void* w_exp_packed, const float* b_exp,
                     const void* w_proj_packed, const float* b_proj_packed, int identity, void* out, int N, int H, int W,
                     int Cin, int Ce, int Co, lp_stream_t stream);
 
+/* ---- M2 block-fused: one stride-2 InvBottleneck (k = 7, no identity) in ONE kernel ------------------------------
+ * Same arithmetic as lp_pw1x1_f16 (ReLU6) -> lp_dwconv_f16 (k7, stride 2, ReLU6, packed fp16) -> lp_pw1x1_f16, values
+ * equal; the 6x tensor never reaches HBM.  x [N,H,W,Cin] fp16 NHWC, H and W even; out [N,H/2,W/2,Co].  Weights as for
+ * lp_block_s1_f16 (w_exp_packed from lp_block_s1_pack_wexp).  Shapes: lp_block_s2_supported() (Cin 8 or 16, Co <= 64,
+ * shared-memory budget on Ce); callers run the three-kernel chain otherwise. */
+int lp_block_s2_supported(int Cin, int Ce, int Co);
+int lp_block_s2_f16(const void* x, const void* w_exp_packed, const float* b_exp, const void* w_dw, const float* b_dw,
+                    const void* w_proj_packed, const float* b_proj_packed, void* out, int N, int H, int W, int Cin,
+                    int Ce, int Co, lp_stream_t stream);
+
 /* ---- M3: fusion deconv level ----------------------------------------------
  * out = ReLU(ConvT4x4s2p1(refined) + ConvT4x4s2p1(raw) + bias), one kernel.
  * refined NHWC fp16 [N,H,W,Cr], raw [N,H,W,Cw], out [N,2H,2W,Co].

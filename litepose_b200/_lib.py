@@ -49,6 +49,8 @@ SIGNATURES = {
     "lp_block_s1_wexp_elems": (_sz, [_i, _i]),
     "lp_block_s1_pack_wexp": (_i, [_vp, _i, _i, _vp]),
     "lp_block_s1_f16": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i, _i, _i, _vp]),
+    "lp_block_s2_supported": (_i, [_i, _i, _i]),
+    "lp_block_s2_f16": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "lp_deconv_packed_elems": (_sz, [_i, _i, _i]),
     "lp_deconv_packed_bias_elems": (_sz, [_i]),
     "lp_deconv_pack": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp]),

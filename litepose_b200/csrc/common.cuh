@@ -176,32 +176,52 @@ __device__ __forceinline__ void wg_mma_chunks(float (&acc)[NC][8], int c0, int n
         if (c >= c0 && c < c0 + nc) wg_mma16(acc[c], ad, wg_desc_sw128(b_addr + (uint32_t)(c - c0) * 2048u));
 }
 
+// The same for operands whose rows are 32 or 64 bytes wide: 8-row swizzle atoms of 256 / 512 bytes stacked along M/N
+// (the layout a TMA box with CU_TENSOR_MAP_SWIZZLE_32B / _64B writes when its inner extent is the row width).
+__device__ __forceinline__ uint64_t wg_desc_sw32(uint32_t smem_addr) {
+    uint64_t d = 0;
+    d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
+    d |= (uint64_t)1 << 16;
+    d |= (uint64_t)(256 >> 4) << 32;               // SBO = 256 B
+    d |= (uint64_t)3 << 62;                        // SWIZZLE_32B
+    return d;
+}
+__device__ __forceinline__ uint64_t wg_desc_sw64(uint32_t smem_addr) {
+    uint64_t d = 0;
+    d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
+    d |= (uint64_t)1 << 16;
+    d |= (uint64_t)(512 >> 4) << 32;               // SBO = 512 B
+    d |= (uint64_t)2 << 62;                        // SWIZZLE_64B
+    return d;
+}
+
 // acc[0..NC) (+)= A[64 rows at a_addr, K=16] x B[16*NC rows at b_addr, K=16]^T as ONE wgmma m64n(16*NC)k16.  The m64nN
 // accumulator fragment is the n16 fragments of its 16-column chunks concatenated in register order (frag_row / frag_col
 // hold per chunk), and the B rows are contiguous 1024-byte swizzle atoms, so this computes what wg_mma_chunks<NC>(acc,
 // 0, NC, ...) does with one A read instead of NC.  accumulate = 0 overwrites acc with the product (scale-d = 0): the
 // accumulators then need no zeroing by ordinary instructions, which would make ptxas fence (and serialise) the wgmma
-// issue when it sits on a data-dependent path.
-template <int NC> __device__ __forceinline__ void wg_mma_n(float (&acc)[NC][8], uint32_t a_addr, uint32_t b_addr, int accumulate = 1);
-template <> __device__ __forceinline__ void wg_mma_n<1>(float (&d)[1][8], uint32_t a_addr, uint32_t b_addr, int accumulate) {
+// issue when it sits on a data-dependent path.  wg_mma_nd takes the two matrix descriptors (any swizzle mode);
+// wg_mma_n builds 128B-swizzle descriptors from shared-memory addresses.
+template <int NC> __device__ __forceinline__ void wg_mma_nd(float (&acc)[NC][8], uint64_t adesc, uint64_t bdesc, int accumulate);
+template <> __device__ __forceinline__ void wg_mma_nd<1>(float (&d)[1][8], uint64_t adesc, uint64_t bdesc, int accumulate) {
     asm volatile(
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
         "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
         : "+f"(d[0][0]), "+f"(d[0][1]), "+f"(d[0][2]), "+f"(d[0][3]), "+f"(d[0][4]), "+f"(d[0][5]), "+f"(d[0][6]), "+f"(d[0][7])
-        : "l"(wg_desc_sw128(a_addr)), "l"(wg_desc_sw128(b_addr)), "r"(accumulate)
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
         : "memory");
 }
-template <> __device__ __forceinline__ void wg_mma_n<2>(float (&d)[2][8], uint32_t a_addr, uint32_t b_addr, int accumulate) {
+template <> __device__ __forceinline__ void wg_mma_nd<2>(float (&d)[2][8], uint64_t adesc, uint64_t bdesc, int accumulate) {
     asm volatile(
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
         "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
         "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
         : "+f"(d[0][0]), "+f"(d[0][1]), "+f"(d[0][2]), "+f"(d[0][3]), "+f"(d[0][4]), "+f"(d[0][5]), "+f"(d[0][6]), "+f"(d[0][7]),
           "+f"(d[1][0]), "+f"(d[1][1]), "+f"(d[1][2]), "+f"(d[1][3]), "+f"(d[1][4]), "+f"(d[1][5]), "+f"(d[1][6]), "+f"(d[1][7])
-        : "l"(wg_desc_sw128(a_addr)), "l"(wg_desc_sw128(b_addr)), "r"(accumulate)
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
         : "memory");
 }
-template <> __device__ __forceinline__ void wg_mma_n<3>(float (&d)[3][8], uint32_t a_addr, uint32_t b_addr, int accumulate) {
+template <> __device__ __forceinline__ void wg_mma_nd<3>(float (&d)[3][8], uint64_t adesc, uint64_t bdesc, int accumulate) {
     asm volatile(
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
         "wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 "
@@ -209,10 +229,10 @@ template <> __device__ __forceinline__ void wg_mma_n<3>(float (&d)[3][8], uint32
         : "+f"(d[0][0]), "+f"(d[0][1]), "+f"(d[0][2]), "+f"(d[0][3]), "+f"(d[0][4]), "+f"(d[0][5]), "+f"(d[0][6]), "+f"(d[0][7]),
           "+f"(d[1][0]), "+f"(d[1][1]), "+f"(d[1][2]), "+f"(d[1][3]), "+f"(d[1][4]), "+f"(d[1][5]), "+f"(d[1][6]), "+f"(d[1][7]),
           "+f"(d[2][0]), "+f"(d[2][1]), "+f"(d[2][2]), "+f"(d[2][3]), "+f"(d[2][4]), "+f"(d[2][5]), "+f"(d[2][6]), "+f"(d[2][7])
-        : "l"(wg_desc_sw128(a_addr)), "l"(wg_desc_sw128(b_addr)), "r"(accumulate)
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
         : "memory");
 }
-template <> __device__ __forceinline__ void wg_mma_n<4>(float (&d)[4][8], uint32_t a_addr, uint32_t b_addr, int accumulate) {
+template <> __device__ __forceinline__ void wg_mma_nd<4>(float (&d)[4][8], uint64_t adesc, uint64_t bdesc, int accumulate) {
     asm volatile(
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
         "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
@@ -222,12 +242,12 @@ template <> __device__ __forceinline__ void wg_mma_n<4>(float (&d)[4][8], uint32
           "+f"(d[1][0]), "+f"(d[1][1]), "+f"(d[1][2]), "+f"(d[1][3]), "+f"(d[1][4]), "+f"(d[1][5]), "+f"(d[1][6]), "+f"(d[1][7]),
           "+f"(d[2][0]), "+f"(d[2][1]), "+f"(d[2][2]), "+f"(d[2][3]), "+f"(d[2][4]), "+f"(d[2][5]), "+f"(d[2][6]), "+f"(d[2][7]),
           "+f"(d[3][0]), "+f"(d[3][1]), "+f"(d[3][2]), "+f"(d[3][3]), "+f"(d[3][4]), "+f"(d[3][5]), "+f"(d[3][6]), "+f"(d[3][7])
-        : "l"(wg_desc_sw128(a_addr)), "l"(wg_desc_sw128(b_addr)), "r"(accumulate)
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
         : "memory");
 }
 
 // m64n80k16 .. m64n160k16: the projection widths of the wide depthwise+projection kernel (dwpw.cu, Co 65..160)
-template <> __device__ __forceinline__ void wg_mma_n<5>(float (&d)[5][8], uint32_t a_addr, uint32_t b_addr, int accumulate) {
+template <> __device__ __forceinline__ void wg_mma_nd<5>(float (&d)[5][8], uint64_t adesc, uint64_t bdesc, int accumulate) {
     asm volatile(
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %42, 0;\n\t"
         "wgmma.mma_async.sync.aligned.m64n80k16.f32.f16.f16 "
@@ -238,10 +258,10 @@ template <> __device__ __forceinline__ void wg_mma_n<5>(float (&d)[5][8], uint32
           "+f"(d[2][0]), "+f"(d[2][1]), "+f"(d[2][2]), "+f"(d[2][3]), "+f"(d[2][4]), "+f"(d[2][5]), "+f"(d[2][6]), "+f"(d[2][7]),
           "+f"(d[3][0]), "+f"(d[3][1]), "+f"(d[3][2]), "+f"(d[3][3]), "+f"(d[3][4]), "+f"(d[3][5]), "+f"(d[3][6]), "+f"(d[3][7]),
           "+f"(d[4][0]), "+f"(d[4][1]), "+f"(d[4][2]), "+f"(d[4][3]), "+f"(d[4][4]), "+f"(d[4][5]), "+f"(d[4][6]), "+f"(d[4][7])
-        : "l"(wg_desc_sw128(a_addr)), "l"(wg_desc_sw128(b_addr)), "r"(accumulate)
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
         : "memory");
 }
-template <> __device__ __forceinline__ void wg_mma_n<6>(float (&d)[6][8], uint32_t a_addr, uint32_t b_addr, int accumulate) {
+template <> __device__ __forceinline__ void wg_mma_nd<6>(float (&d)[6][8], uint64_t adesc, uint64_t bdesc, int accumulate) {
     asm volatile(
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
         "wgmma.mma_async.sync.aligned.m64n96k16.f32.f16.f16 "
@@ -253,10 +273,10 @@ template <> __device__ __forceinline__ void wg_mma_n<6>(float (&d)[6][8], uint32
           "+f"(d[3][0]), "+f"(d[3][1]), "+f"(d[3][2]), "+f"(d[3][3]), "+f"(d[3][4]), "+f"(d[3][5]), "+f"(d[3][6]), "+f"(d[3][7]),
           "+f"(d[4][0]), "+f"(d[4][1]), "+f"(d[4][2]), "+f"(d[4][3]), "+f"(d[4][4]), "+f"(d[4][5]), "+f"(d[4][6]), "+f"(d[4][7]),
           "+f"(d[5][0]), "+f"(d[5][1]), "+f"(d[5][2]), "+f"(d[5][3]), "+f"(d[5][4]), "+f"(d[5][5]), "+f"(d[5][6]), "+f"(d[5][7])
-        : "l"(wg_desc_sw128(a_addr)), "l"(wg_desc_sw128(b_addr)), "r"(accumulate)
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
         : "memory");
 }
-template <> __device__ __forceinline__ void wg_mma_n<7>(float (&d)[7][8], uint32_t a_addr, uint32_t b_addr, int accumulate) {
+template <> __device__ __forceinline__ void wg_mma_nd<7>(float (&d)[7][8], uint64_t adesc, uint64_t bdesc, int accumulate) {
     asm volatile(
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %58, 0;\n\t"
         "wgmma.mma_async.sync.aligned.m64n112k16.f32.f16.f16 "
@@ -270,10 +290,10 @@ template <> __device__ __forceinline__ void wg_mma_n<7>(float (&d)[7][8], uint32
           "+f"(d[4][0]), "+f"(d[4][1]), "+f"(d[4][2]), "+f"(d[4][3]), "+f"(d[4][4]), "+f"(d[4][5]), "+f"(d[4][6]), "+f"(d[4][7]),
           "+f"(d[5][0]), "+f"(d[5][1]), "+f"(d[5][2]), "+f"(d[5][3]), "+f"(d[5][4]), "+f"(d[5][5]), "+f"(d[5][6]), "+f"(d[5][7]),
           "+f"(d[6][0]), "+f"(d[6][1]), "+f"(d[6][2]), "+f"(d[6][3]), "+f"(d[6][4]), "+f"(d[6][5]), "+f"(d[6][6]), "+f"(d[6][7])
-        : "l"(wg_desc_sw128(a_addr)), "l"(wg_desc_sw128(b_addr)), "r"(accumulate)
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
         : "memory");
 }
-template <> __device__ __forceinline__ void wg_mma_n<8>(float (&d)[8][8], uint32_t a_addr, uint32_t b_addr, int accumulate) {
+template <> __device__ __forceinline__ void wg_mma_nd<8>(float (&d)[8][8], uint64_t adesc, uint64_t bdesc, int accumulate) {
     asm volatile(
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
         "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
@@ -288,10 +308,10 @@ template <> __device__ __forceinline__ void wg_mma_n<8>(float (&d)[8][8], uint32
           "+f"(d[5][0]), "+f"(d[5][1]), "+f"(d[5][2]), "+f"(d[5][3]), "+f"(d[5][4]), "+f"(d[5][5]), "+f"(d[5][6]), "+f"(d[5][7]),
           "+f"(d[6][0]), "+f"(d[6][1]), "+f"(d[6][2]), "+f"(d[6][3]), "+f"(d[6][4]), "+f"(d[6][5]), "+f"(d[6][6]), "+f"(d[6][7]),
           "+f"(d[7][0]), "+f"(d[7][1]), "+f"(d[7][2]), "+f"(d[7][3]), "+f"(d[7][4]), "+f"(d[7][5]), "+f"(d[7][6]), "+f"(d[7][7])
-        : "l"(wg_desc_sw128(a_addr)), "l"(wg_desc_sw128(b_addr)), "r"(accumulate)
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
         : "memory");
 }
-template <> __device__ __forceinline__ void wg_mma_n<9>(float (&d)[9][8], uint32_t a_addr, uint32_t b_addr, int accumulate) {
+template <> __device__ __forceinline__ void wg_mma_nd<9>(float (&d)[9][8], uint64_t adesc, uint64_t bdesc, int accumulate) {
     asm volatile(
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %74, 0;\n\t"
         "wgmma.mma_async.sync.aligned.m64n144k16.f32.f16.f16 "
@@ -307,10 +327,10 @@ template <> __device__ __forceinline__ void wg_mma_n<9>(float (&d)[9][8], uint32
           "+f"(d[6][0]), "+f"(d[6][1]), "+f"(d[6][2]), "+f"(d[6][3]), "+f"(d[6][4]), "+f"(d[6][5]), "+f"(d[6][6]), "+f"(d[6][7]),
           "+f"(d[7][0]), "+f"(d[7][1]), "+f"(d[7][2]), "+f"(d[7][3]), "+f"(d[7][4]), "+f"(d[7][5]), "+f"(d[7][6]), "+f"(d[7][7]),
           "+f"(d[8][0]), "+f"(d[8][1]), "+f"(d[8][2]), "+f"(d[8][3]), "+f"(d[8][4]), "+f"(d[8][5]), "+f"(d[8][6]), "+f"(d[8][7])
-        : "l"(wg_desc_sw128(a_addr)), "l"(wg_desc_sw128(b_addr)), "r"(accumulate)
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
         : "memory");
 }
-template <> __device__ __forceinline__ void wg_mma_n<10>(float (&d)[10][8], uint32_t a_addr, uint32_t b_addr, int accumulate) {
+template <> __device__ __forceinline__ void wg_mma_nd<10>(float (&d)[10][8], uint64_t adesc, uint64_t bdesc, int accumulate) {
     asm volatile(
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %82, 0;\n\t"
         "wgmma.mma_async.sync.aligned.m64n160k16.f32.f16.f16 "
@@ -328,8 +348,13 @@ template <> __device__ __forceinline__ void wg_mma_n<10>(float (&d)[10][8], uint
           "+f"(d[7][0]), "+f"(d[7][1]), "+f"(d[7][2]), "+f"(d[7][3]), "+f"(d[7][4]), "+f"(d[7][5]), "+f"(d[7][6]), "+f"(d[7][7]),
           "+f"(d[8][0]), "+f"(d[8][1]), "+f"(d[8][2]), "+f"(d[8][3]), "+f"(d[8][4]), "+f"(d[8][5]), "+f"(d[8][6]), "+f"(d[8][7]),
           "+f"(d[9][0]), "+f"(d[9][1]), "+f"(d[9][2]), "+f"(d[9][3]), "+f"(d[9][4]), "+f"(d[9][5]), "+f"(d[9][6]), "+f"(d[9][7])
-        : "l"(wg_desc_sw128(a_addr)), "l"(wg_desc_sw128(b_addr)), "r"(accumulate)
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
         : "memory");
+}
+
+template <int NC>
+__device__ __forceinline__ void wg_mma_n(float (&acc)[NC][8], uint32_t a_addr, uint32_t b_addr, int accumulate = 1) {
+    wg_mma_nd<NC>(acc, wg_desc_sw128(a_addr), wg_desc_sw128(b_addr), accumulate);
 }
 
 // Accumulator fragment of m64n16 per thread (warp w = warp % 4 of the warpgroup): value pair i (0..3) of chunk c is

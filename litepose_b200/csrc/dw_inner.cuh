@@ -18,12 +18,14 @@ namespace lp {
 
 // PP = pixel pitch of the slab in half2 units: CB/2 for the pixel-major [I][I][CB] slab the TMA delivers (dwpw.cu,
 // tile_in already offset by the thread's channel pair), 4 for the chunk-major slab of dwblock.cu
-// ([4 chunks of 8 channels][I*I pixels][16 B], tile_in offset by chunk base + pair inside the chunk).
-template <int K, int BY, int I, int CB, int PP = CB / 2>
+// ([4 chunks of 8 channels][I*I pixels][16 B], tile_in offset by chunk base + pair inside the chunk), any other pitch
+// with tile_in offset by the pair.  I = row pitch of the slab in pixels.  S = stride: output (oy + i, ox + j) reads
+// input (S (oy + i) + ky, S (ox + j) + kx) of the slab.  Stride 2 has no mirrored lanes (mir must be false).
+template <int K, int BY, int I, int CB, int PP = CB / 2, int S = 1>
 __device__ __forceinline__ void dw_slab_hfma2(const __half2* __restrict__ tile_in, const __half2* __restrict__ wslab, int cp,
                                               bool mir, int oy, int ox, __half2 bias, __half2 (&acc)[BY][4]) {
-    constexpr int IRX = 4 + K - 1;       // input columns of a micro-block
-    constexpr int IRY = BY + K - 1;      // input rows
+    constexpr int IRX = 3 * S + K;       // input columns of a micro-block
+    constexpr int IRY = (BY - 1) * S + K;   // input rows
     constexpr int HP = CB / 2;           // half2 per pixel of the weight slab
     const int cstep = mir ? -PP : PP;
     __half2 part[BY][4];
@@ -40,7 +42,7 @@ __device__ __forceinline__ void dw_slab_hfma2(const __half2* __restrict__ tile_i
 #pragma unroll
             for (int kx = 0; kx < K; ++kx) wreg[ky * K + kx] = ws[ky * K * HP + kx * wstep];
     }
-    const __half2* base = tile_in + (oy * I + ox + (mir ? IRX - 1 : 0)) * PP + (PP == HP ? cp : 0);
+    const __half2* base = tile_in + (S * (oy * I + ox) + (mir ? IRX - 1 : 0)) * PP + (PP == HP ? cp : 0);
 #pragma unroll
     for (int r = 0; r < IRY; ++r) {
         __half2 in[IRX];
@@ -48,15 +50,15 @@ __device__ __forceinline__ void dw_slab_hfma2(const __half2* __restrict__ tile_i
         for (int c = 0; c < IRX; ++c) in[c] = base[r * I * PP + c * cstep];
 #pragma unroll
         for (int i = 0; i < BY; ++i) {
-            const int ky = r - i;
+            const int ky = r - i * S;
             if (ky >= 0 && ky < K) {
 #pragma unroll
                 for (int kx = 0; kx < K; ++kx) {
                     const __half2 wv = wreg[ky * K + kx];
 #pragma unroll
                     for (int j = 0; j < 4; ++j) {
-                        if ((ky & 1) == 0 && kx == 0) part[i][j] = __hmul2(in[j + kx], wv);     // a new two-row chain
-                        else part[i][j] = __hfma2(in[j + kx], wv, part[i][j]);
+                        if ((ky & 1) == 0 && kx == 0) part[i][j] = __hmul2(in[j * S + kx], wv);     // a new two-row chain
+                        else part[i][j] = __hfma2(in[j * S + kx], wv, part[i][j]);
                     }
                 }
                 if ((ky & 1) || ky == K - 1) {

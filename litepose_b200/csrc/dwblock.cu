@@ -353,6 +353,277 @@ block_s1_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
     }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// One stride-2 inverted-residual block (k = 7, Cin <= 16, no identity) in ONE kernel: the same arithmetic as
+// lp_pw1x1_f16 (ReLU6) -> lp_dwconv_f16 (k7, s2, ReLU6, packed fp16) -> lp_pw1x1_f16, without the 6x tensor in HBM.
+// Per 16x8-pixel output tile (one 128-row projection M-tile pair) the CTA
+//   * TMA-loads the haloed input X [21 rows][37 px][16 ch] at its real width: 777 rows of 32 B, 32B-swizzled, channels
+//     beyond Cin and pixels outside the image zero-filled by the tensor map,
+//   * per 32-channel slab: expands X on the tensor cores (14 x wgmma m64n32k16, one K=16 slice), + bias -> fp16 -> ReLU6,
+//     zero outside the image, into a pixel-major [777 px][32 ch] slab with a 72-byte pixel pitch, then runs the packed
+//     fp16 7x7 stride-2 depthwise of dw_inner.cuh on it (thread = channel pair x 4x4 output micro-block) and writes the
+//     ReLU6'd results into the slab's 64B-swizzled A tile [128 px][32 ch],
+//   * projects all slabs at once: warpgroup w runs output rows 4w..4w+3 (M = 64) over every K=16 slice in channel order,
+//     4 slices per 64-channel K block like lp_pw1x1_f16 (the slices past Ce read zero A rows against zero weights),
+//     fp32 accumulators, + bias, one rounding to fp16.
+// Warp roles: two warpgroups, each expands and convolves its own slabs (s = wg, wg + 2, ...) with its own slab buffer;
+// an odd last slab is shared (expansion by M-tile halves, depthwise on 4x2 micro-blocks, both in warpgroup 0's buffer),
+// and named barrier, so one warpgroup's expansion epilogue overlaps the other's depthwise loop.  Thread 0 also issues
+// the TMA loads: the next tile's X as soon as every warp has expanded its last slab of the current tile.
+// Bank conflicts: the two half-warps of a warp convolve x-adjacent micro-blocks, i.e. read pixels 8 apart; with
+// 72-byte pixels those are 144 words apart (= 16 mod 32 banks), so the 16 + 16 words of one LDS fall into 32 banks.
+// HBM traffic: read N*H*W*Cin*2 (plus halo re-reads, L2 hits), write N*H/2*W/2*Co*2.
+constexpr int S2_TW = 16, S2_TH = 8;                       // output tile
+constexpr int S2_IW = 2 * S2_TW + 5, S2_IH = 2 * S2_TH + 5; // haloed input tile: 37 x 21
+constexpr int S2_PIX = S2_IW * S2_IH;                       // 777 rows of X / pixels of a slab
+constexpr int S2_X_BYTES = 14 * 64 * 32;                    // 14 M-tiles of 64 rows x 32 B (TMA fills the first 777 rows)
+constexpr int S2_X_TX = S2_PIX * 32;
+constexpr int S2_PP = 18;                                   // slab pixel pitch in half2 (72 B)
+constexpr int S2_SLAB = (S2_PIX * S2_PP * 4 + 127) & ~127;  // 56064 B
+constexpr int S2_WE_SLAB = 32 * 32;                         // expansion weights of a slab: 32 rows x 32 B
+constexpr int S2_A_SLAB = 128 * 64;                         // A tile of a slab: 128 px x 64 B
+constexpr int S2_THREADS = 256;
+
+struct S2Bars {
+    uint64_t w_full, x_full, x_empty;
+};
+
+struct S2Params {
+    int N, H, W, Cin, Ce, Co, Hout, Wout, n_tile;
+    int tiles_x, tiles_y, num_tiles;
+    int nslabs, nkb;
+    int off_we, off_a, off_wp, off_slab, off_dww, off_bias;
+    const float* b_exp;               // [Ce]
+    const float* b_dw;                // [Ce]
+    const float* b_pj;                // packed, n_tile
+    __half* out;                      // [N,H/2,W/2,Co]
+};
+
+// next tile's haloed input into sX, once every warp has expanded its last slab of tile `it`
+__device__ __forceinline__ void s2_load_next_x(const CUtensorMap* map_x, S2Bars* bars, uint8_t* sX, const S2Params& p, int t2,
+                                               int it) {
+    if (t2 >= p.num_tiles) return;
+    const int tx = t2 % p.tiles_x, ty = (t2 / p.tiles_x) % p.tiles_y, n = t2 / (p.tiles_x * p.tiles_y);
+    mbar_wait(&bars->x_empty, it & 1);
+    mbar_expect_tx(&bars->x_full, S2_X_TX);
+    tma_load_4d(sX, map_x, &bars->x_full, 0, tx * 2 * S2_TW - 3, ty * 2 * S2_TH - 3, n);
+}
+
+// expansion of slab s into `slab` for haloed pixels of M-tiles 2 mp0 .. 2 mp1 - 1 (one warpgroup, two M-tiles per
+// wgmma batch): + bias in fp32, round to fp16, ReLU6 (clamping commutes with rounding), zero outside the image
+__device__ __forceinline__ void s2_expand(uint8_t* slab, const uint8_t* sX, const uint8_t* sWe, const float* sBexp, int s,
+                                          int mp0, int mp1, uint32_t in_img, int wq, int lane) {
+    const __half2 zero2 = __floats2half2_rn(0.f, 0.f), six2 = __floats2half2_rn(6.f, 6.f);
+    float be[2][2][2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+            const int ch = c * 16 + frag_col(lane, 2 * i);
+            be[i][c][0] = sBexp[s * BK_CB + ch];
+            be[i][c][1] = sBexp[s * BK_CB + ch + 1];
+        }
+    const uint64_t bdesc = wg_desc_sw32(smem_u32(sWe + s * S2_WE_SLAB));
+#pragma unroll 1
+    for (int mp = mp0; mp < mp1; ++mp) {
+        float eacc[2][2][8];
+        wg_fence();
+#pragma unroll
+        for (int b = 0; b < 2; ++b) wg_mma_nd<2>(eacc[b], wg_desc_sw32(smem_u32(sX) + (mp * 2 + b) * 2048), bdesc, 0);
+        wg_commit();
+        wg_wait0();
+#pragma unroll
+        for (int b = 0; b < 2; ++b)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int pi = (mp * 2 + b) * 64 + frag_row(wq, lane, i);
+                if (pi >= S2_PIX) continue;
+                const bool in = (in_img >> ((mp * 2 + b) * 2 + (i & 1))) & 1;
+#pragma unroll
+                for (int c = 0; c < 2; ++c) {
+                    const int ch = c * 16 + frag_col(lane, i);
+                    __half2 h = zero2;
+                    if (in)
+                        h = __hmin2(__hmax2(__floats2half2_rn(eacc[b][c][2 * i] + be[i >> 1][c][0],
+                                                              eacc[b][c][2 * i + 1] + be[i >> 1][c][1]),
+                                            zero2),
+                                    six2);
+                    *reinterpret_cast<__half2*>(slab + pi * (S2_PP * 4) + ch * 2) = h;
+                }
+            }
+    }
+}
+
+// depthwise 7x7 stride 2 of slab s (dw_inner.cuh) for the thread's channel pair and 4-wide x BY-tall micro-block at
+// (oy, ox) of the output tile, ReLU6, into the slab's 64B-swizzled A tile (row = pixel of the 16x8 tile)
+template <int BY>
+__device__ __forceinline__ void s2_depthwise(const uint8_t* slab, const uint8_t* sDww, const float* sBdw, uint8_t* sA, int s,
+                                             int cp, int oy, int ox) {
+    const __half2 zero2 = __floats2half2_rn(0.f, 0.f), six2 = __floats2half2_rn(6.f, 6.f);
+    __half2 acch[BY][4];
+    const __half2 bh = __float22half2_rn(*reinterpret_cast<const float2*>(sBdw + s * BK_CB + 2 * cp));
+    dw_slab_hfma2<7, BY, S2_IW, BK_CB, S2_PP, 2>(reinterpret_cast<const __half2*>(slab) + cp,
+                                                 reinterpret_cast<const __half2*>(sDww + s * BK_DW_SLAB), cp, false, oy, ox,
+                                                 bh, acch);
+    uint8_t* a_s = sA + s * S2_A_SLAB;
+#pragma unroll
+    for (int i = 0; i < BY; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int r = (oy + i) * S2_TW + ox + j;
+            const __half2 v = __hmin2(__hmax2(acch[i][j], zero2), six2);
+            *reinterpret_cast<__half2*>(a_s + r * 64 + (((cp >> 2) ^ ((r >> 1) & 3)) << 4) + ((cp & 3) << 2)) = v;
+        }
+}
+
+// NC = n_tile / 16 projection chunks (one m64n(16 NC)k16 per K=16 slice)
+template <int NC>
+__global__ void __launch_bounds__(S2_THREADS, 1)
+block_s2_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_we,
+                const __grid_constant__ CUtensorMap map_dw, const __grid_constant__ CUtensorMap map_wp,
+                const __grid_constant__ S2Params p) {
+    extern __shared__ __align__(1024) uint8_t smem[];
+    uint8_t* sX = smem;
+    uint8_t* sWe = smem + p.off_we;
+    uint8_t* sA = smem + p.off_a;
+    uint8_t* sWp = smem + p.off_wp;
+    uint8_t* sDww = smem + p.off_dww;
+    float* sBexp = reinterpret_cast<float*>(smem + p.off_bias);
+    float* sBdw = sBexp + p.nslabs * 32;
+    float* sBpj = sBdw + p.nslabs * 32;
+    S2Bars* bars = reinterpret_cast<S2Bars*>(sBpj + 64);
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = warp >> 2, wq = warp & 3;
+    uint8_t* slab = smem + p.off_slab + wg * S2_SLAB;
+
+    if (threadIdx.x == 0) {
+        tma_prefetch_desc(&map_x);
+        tma_prefetch_desc(&map_we);
+        tma_prefetch_desc(&map_dw);
+        tma_prefetch_desc(&map_wp);
+        mbar_init(&bars->w_full, 1);
+        mbar_init(&bars->x_full, 1);
+        mbar_init(&bars->x_empty, S2_THREADS / 32);
+        fence_barrier_init();
+    }
+    for (int i = threadIdx.x; i < p.nslabs * 32; i += S2_THREADS) {
+        sBexp[i] = (i < p.Ce && p.b_exp) ? p.b_exp[i] : 0.f;
+        sBdw[i] = (i < p.Ce && p.b_dw) ? p.b_dw[i] : 0.f;
+    }
+    for (int i = threadIdx.x; i < p.n_tile; i += S2_THREADS) sBpj[i] = p.b_pj ? p.b_pj[i] : 0.f;
+    // A tiles of the slabs past the last one (the rest of the last K block) stay zero
+    for (int i = p.nslabs * S2_A_SLAB / 16 + threadIdx.x; i < 2 * p.nkb * S2_A_SLAB / 16; i += S2_THREADS)
+        reinterpret_cast<uint4*>(sA)[i] = make_uint4(0, 0, 0, 0);
+    fence_proxy_async();
+    pdl_launch_dependents();
+    __syncthreads();
+
+    if (threadIdx.x == 0) {
+        // weights are static: they may be fetched before the previous kernel of the stream has finished
+        mbar_expect_tx(&bars->w_full, (uint32_t)(p.nslabs * (S2_WE_SLAB + BK_DW_BYTES) + p.nkb * p.n_tile * 128));
+        for (int s = 0; s < p.nslabs; ++s) {
+            tma_load_2d(sWe + s * S2_WE_SLAB, &map_we, &bars->w_full, 0, s * BK_CB);
+            tma_load_2d(sDww + s * BK_DW_SLAB, &map_dw, &bars->w_full, s * BK_CB, 0);
+        }
+        for (int kb = 0; kb < p.nkb; ++kb) tma_load_2d(sWp + kb * p.n_tile * 128, &map_wp, &bars->w_full, 0, kb * p.n_tile);
+    }
+    pdl_wait();                       // the block input is complete from here on (and the output no longer read)
+    if (threadIdx.x == 0 && (int)blockIdx.x < p.num_tiles) {
+        const int t = blockIdx.x;
+        const int tx = t % p.tiles_x, ty = (t / p.tiles_x) % p.tiles_y, n = t / (p.tiles_x * p.tiles_y);
+        mbar_expect_tx(&bars->x_full, S2_X_TX);
+        tma_load_4d(sX, &map_x, &bars->x_full, 0, tx * 2 * S2_TW - 3, ty * 2 * S2_TH - 3, n);
+    }
+    mbar_wait(&bars->w_full, 0);
+
+    const int cp = threadIdx.x & 15;
+    const int blk = (wq << 1) | ((threadIdx.x >> 4) & 1);       // micro-block of the 4 x 2 grid of 4x4 blocks
+    const int oy = (blk >> 2) * 4, ox = (blk & 3) * 4;
+    const int nk16 = 4 * p.nkb;
+    float pacc[NC][8];
+    int it = 0;
+    for (int t = blockIdx.x; t < p.num_tiles; t += gridDim.x, ++it) {
+        const int tx = t % p.tiles_x, ty = (t / p.tiles_x) % p.tiles_y, n = t / (p.tiles_x * p.tiles_y);
+        // which of the thread's 28 expansion rows (M-tile m, rows frag_row(wq, lane, 0 / 1)) lie inside the image
+        uint32_t in_img = 0;
+#pragma unroll
+        for (int m = 0; m < 14; ++m)
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const int pi = m * 64 + frag_row(wq, lane, i);
+                const int yy = pi / S2_IW, xx = pi - yy * S2_IW;
+                const int gy = ty * 2 * S2_TH - 3 + yy, gx = tx * 2 * S2_TW - 3 + xx;
+                if (pi < S2_PIX && gy >= 0 && gy < p.H && gx >= 0 && gx < p.W) in_img |= 1u << (m * 2 + i);
+            }
+        mbar_wait(&bars->x_full, it & 1);
+        // Slabs 0 .. nfull-1 alternate between the warpgroups; an odd last slab is split between both (expansion by
+        // M-tile halves, depthwise on 4x2 micro-blocks), so that neither warpgroup idles for a whole slab.
+        const int nfull = p.nslabs & ~1;
+        for (int s = wg; s < nfull; s += 2) {
+            asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");   // the previous slab is fully consumed
+            s2_expand(slab, sX, sWe, sBexp, s, 0, 7, in_img, wq, lane);
+            const bool last = s + 2 >= nfull && nfull == p.nslabs;
+            if (last) {
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&bars->x_empty);                   // X may be overwritten
+            }
+            asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");   // slab complete
+            if (last && threadIdx.x == 0) s2_load_next_x(&map_x, bars, sX, p, t + gridDim.x, it);
+            s2_depthwise<4>(slab, sDww, sBdw, sA, s, cp, oy, ox);
+        }
+        if (nfull < p.nslabs) {
+            const int s = nfull;
+            uint8_t* slab0 = smem + p.off_slab;
+            asm volatile("bar.sync 3, 256;" ::: "memory");                  // warpgroup 0's slab buffer is free
+            s2_expand(slab0, sX, sWe, sBexp, s, wg ? 4 : 0, wg ? 7 : 4, in_img, wq, lane);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&bars->x_empty);
+            asm volatile("bar.sync 3, 256;" ::: "memory");                  // slab complete
+            if (threadIdx.x == 0) s2_load_next_x(&map_x, bars, sX, p, t + gridDim.x, it);
+            const int b16 = (wg << 3) | blk;                                // 16 micro-blocks of 4 x 2 rows
+            s2_depthwise<2>(slab0, sDww, sBdw, sA, s, cp, (b16 >> 2) * 2, (b16 & 3) * 4);
+        }
+        fence_proxy_async();
+        __syncthreads();                                                     // A complete
+        // ---- projection: warpgroup wg = output rows 4 wg .. 4 wg + 3, every K=16 slice in channel order
+        const uint32_t a_base = smem_u32(sA) + wg * 64 * 64;
+        const uint32_t b_base = smem_u32(sWp);
+        wg_fence();
+        for (int k = 0; k < nk16; ++k)
+            wg_mma_nd<NC>(pacc, wg_desc_sw64(a_base + (k >> 1) * S2_A_SLAB + (k & 1) * 32),
+                          wg_desc_sw128(b_base + (k >> 2) * p.n_tile * 128 + (k & 3) * 32), k);
+        wg_commit();
+        wg_wait0();
+        __syncthreads();                                                     // A may be overwritten
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int row = wg * 64 + frag_row(wq, lane, i);
+            const int gy = ty * S2_TH + (row >> 4), gx = tx * S2_TW + (row & 15);
+            if (gy >= p.Hout || gx >= p.Wout) continue;
+            const size_t off = (((size_t)n * p.Hout + gy) * p.Wout + gx) * p.Co;
+#pragma unroll
+            for (int c = 0; c < NC; ++c) {
+                const int co = c * 16 + frag_col(lane, i);
+                if (co >= p.Co) continue;
+                *reinterpret_cast<__half2*>(p.out + off + co) =
+                    __float22half2_rn(make_float2(pacc[c][2 * i] + sBpj[co], pacc[c][2 * i + 1] + sBpj[co + 1]));
+            }
+        }
+    }
+}
+
+static size_t s2_layout(S2Params& p) {
+    size_t off = S2_X_BYTES;                                                  // 1024-aligned (28 KiB)
+    p.off_we = (int)off;    off += ((size_t)p.nslabs * S2_WE_SLAB + 1023) & ~(size_t)1023;
+    p.off_a = (int)off;     off += (size_t)2 * p.nkb * S2_A_SLAB;            // 8 KiB per slab, 1024-aligned
+    p.off_wp = (int)off;    off += ((size_t)p.nkb * p.n_tile * 128 + 1023) & ~(size_t)1023;
+    p.off_slab = (int)off;  off += 2 * S2_SLAB;
+    p.off_dww = (int)off;   off += ((size_t)p.nslabs * BK_DW_SLAB + 127) & ~(size_t)127;
+    p.off_bias = (int)off;  off += ((size_t)2 * p.nslabs * 32 + 64) * 4 + sizeof(S2Bars) + 64;
+    return off + 1024;                                                        // alignment slack of the dynamic base
+}
+
 static size_t bk_layout(BkParams& p, int stream) {
     size_t off = BK_X_BYTES;
     const int n_we = stream ? 2 : p.nslabs, n_dw = stream ? 4 : p.nslabs;
@@ -474,5 +745,82 @@ extern "C" int lp_block_s1_f16(const void* x, const void* w_exp_packed, const fl
     e = launch_pdl(k, dim3(grid), dim3(BK_THREADS), (size_t)need, (cudaStream_t)stream, mx, mwe, mdw, mwp, p);
     if (e != cudaSuccess) return cuda_fail(e, "launch block_s1_kernel");
     LP_LAUNCH_CHECK("block_s1_kernel");
+    return LP_OK;
+}
+
+static int s2_shape_ok(int Cin, int Ce, int Co, S2Params* out) {
+    if (Cin < 8 || Cin > 16 || Cin % 8 || Ce < 8 || Ce % 8 || Co < 8 || Co % 8 || Co > 64) return 0;
+    S2Params p;
+    memset(&p, 0, sizeof(p));
+    p.Cin = Cin; p.Ce = Ce; p.Co = Co;
+    p.n_tile = (Co + 15) / 16 * 16;
+    p.nslabs = (Ce + BK_CB - 1) / BK_CB;
+    p.nkb = (Ce + 63) / 64;
+    const size_t need = s2_layout(p);
+    if (need > 232448) return 0;                 // 227 KiB of dynamic shared memory per CTA on sm_90
+    if (out) *out = p;
+    return (int)need;
+}
+
+// 1 when lp_block_s2_f16 can run this block shape (Cin <= 16, Co <= 64, shared-memory budget on Ce), else 0
+extern "C" int lp_block_s2_supported(int Cin, int Ce, int Co) { return s2_shape_ok(Cin, Ce, Co, nullptr) > 0; }
+
+// x [N,H,W,Cin] fp16 NHWC -> out [N,H/2,W/2,Co]: relu6(x We^T + be) -> dw7x7 stride 2 (+bd, relu6) -> Wp (+bp)
+extern "C" int lp_block_s2_f16(const void* x, const void* w_exp_packed, const float* b_exp, const void* w_dw,
+                               const float* b_dw, const void* w_proj_packed, const float* b_proj_packed, void* out, int N,
+                               int H, int W, int Cin, int Ce, int Co, lp_stream_t stream) {
+    LP_CHECK_ARG(x && w_exp_packed && w_dw && w_proj_packed && out, "lp_block_s2_f16: null pointer");
+    S2Params p;
+    const int need = s2_shape_ok(Cin, Ce, Co, &p);
+    LP_CHECK_ARG(N > 0 && H > 0 && W > 0 && H % 2 == 0 && W % 2 == 0 && need > 0,
+                 "lp_block_s2_f16: unsupported shape N=%d H=%d W=%d Cin=%d Ce=%d Co=%d (even H, W; see "
+                 "lp_block_s2_supported)", N, H, W, Cin, Ce, Co);
+    if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(w_proj_packed) |
+         reinterpret_cast<uintptr_t>(w_exp_packed) | reinterpret_cast<uintptr_t>(w_dw)) & 15) {
+        set_error("lp_block_s2_f16: pointers must be 16-byte aligned");
+        return LP_ERR_ALIGN;
+    }
+    p.N = N; p.H = H; p.W = W;
+    p.Hout = H / 2; p.Wout = W / 2;
+    p.tiles_x = (p.Wout + S2_TW - 1) / S2_TW;
+    p.tiles_y = (p.Hout + S2_TH - 1) / S2_TH;
+    p.num_tiles = p.tiles_x * p.tiles_y * N;
+    p.b_exp = b_exp;
+    p.b_dw = b_dw;
+    p.b_pj = b_proj_packed;
+    p.out = reinterpret_cast<__half*>(out);
+    CUtensorMap mx, mwe, mdw, mwp;
+    {
+        uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)N};
+        uint64_t strides[3] = {(uint64_t)Cin * 2, (uint64_t)W * Cin * 2, (uint64_t)H * W * Cin * 2};
+        uint32_t box[4] = {16u, (uint32_t)S2_IW, (uint32_t)S2_IH, 1u};
+        int rc = make_tmap(&mx, x, 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_32B);
+        if (rc) return rc;
+        // the K = 16 slice (columns 0..15) of lp_block_s1_pack_wexp's [nslabs*32][64] rows
+        uint64_t d2[2] = {64u, (uint64_t)p.nslabs * BK_CB};
+        uint64_t s2[1] = {128u};
+        uint32_t b2[2] = {16u, (uint32_t)BK_CB};
+        rc = make_tmap(&mwe, w_exp_packed, 2, d2, s2, b2, CU_TENSOR_MAP_SWIZZLE_32B);
+        if (rc) return rc;
+        uint64_t d3[2] = {(uint64_t)Ce, 49u};
+        uint64_t s3[1] = {(uint64_t)Ce * 2};
+        uint32_t b3[2] = {(uint32_t)BK_CB, 49u};
+        rc = make_tmap(&mdw, w_dw, 2, d3, s3, b3, CU_TENSOR_MAP_SWIZZLE_NONE);
+        if (rc) return rc;
+        uint64_t d4[2] = {64u, (uint64_t)p.nkb * p.n_tile};
+        uint64_t s4[1] = {128u};
+        uint32_t b4[2] = {64u, (uint32_t)p.n_tile};
+        rc = make_tmap(&mwp, w_proj_packed, 2, d4, s4, b4, CU_TENSOR_MAP_SWIZZLE_128B);
+        if (rc) return rc;
+    }
+    const int grid = p.num_tiles < num_sms() ? p.num_tiles : num_sms();
+    using Kern = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const S2Params);
+    static const Kern kernels[4] = {block_s2_kernel<1>, block_s2_kernel<2>, block_s2_kernel<3>, block_s2_kernel<4>};
+    const Kern k = kernels[p.n_tile / 16 - 1];
+    cudaError_t e = cudaFuncSetAttribute((const void*)k, cudaFuncAttributeMaxDynamicSharedMemorySize, need);
+    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(block_s2)");
+    e = launch_pdl(k, dim3(grid), dim3(S2_THREADS), (size_t)need, (cudaStream_t)stream, mx, mwe, mdw, mwp, p);
+    if (e != cudaSuccess) return cuda_fail(e, "launch block_s2_kernel");
+    LP_LAUNCH_CHECK("block_s2_kernel");
     return LP_OK;
 }

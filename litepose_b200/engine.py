@@ -208,8 +208,10 @@ class LitePoseEngine(object):
                 s, b = _fold(sd, p + "point_conv.1")
                 pc = self._pack_pw(sd[p + "point_conv.0.weight"].float() * s.view(-1, 1, 1, 1), b)
                 cin, cout = inv["K"], pc["N"]
-                if stride == 1 and dw["k"] == 7 and self.lib.lp_block_s1_supported(cin, inv["N"], cout):
-                    # block-fused kernel: expansion weights as [Ce][Cin padded to 64] K-major rows, fp32 bias
+                if dw["k"] == 7 and ((stride == 1 and self.lib.lp_block_s1_supported(cin, inv["N"], cout)) or
+                                     (stride == 2 and self.lib.lp_block_s2_supported(cin, inv["N"], cout))):
+                    # block-fused kernel (lp_block_s1_f16 / lp_block_s2_f16): expansion weights as [Ce][Cin padded to
+                    # 64] K-major rows, fp32 bias
                     wfold = sd[p + "inv.0.weight"].float() * _fold(sd, p + "inv.1")[0].view(-1, 1, 1, 1)
                     w16 = _np16(wfold.reshape(inv["N"], cin))
                     wk = np.zeros(self.lib.lp_block_s1_wexp_elems(cin, inv["N"]), np.uint16)
@@ -302,17 +304,17 @@ class LitePoseEngine(object):
                                                           x0.data_ptr(), n * h2 * w2, q["K"], q["N"], _lib.ACT_NONE]))
         x_list = [(x0, h2, w2)]
         cur, ch, cw_ = x0, h2, w2
-        # scratch for the expanded tensors, sized for the largest block
+        # scratch for the expanded tensors, sized for the largest block that does not run as one kernel
         max_e = max_d = 0
         th, tw = h2, w2
         for blk in P["blocks"]:
-            e = n * th * tw * blk["inv"]["N"]
             th2, tw2 = th // blk["stride"], tw // blk["stride"]
-            max_e = max(max_e, e)
-            max_d = max(max_d, n * th2 * tw2 * blk["dw"]["C"])
+            if "wblk" not in blk["inv"]:
+                max_e = max(max_e, n * th * tw * blk["inv"]["N"])
+                max_d = max(max_d, n * th2 * tw2 * blk["dw"]["C"])
             th, tw = th2, tw2
-        e_buf = alloc((max_e,), f16)
-        d_buf = alloc((max_d,), f16)
+        e_buf = alloc((max(max_e, 1),), f16)
+        d_buf = alloc((max(max_d, 1),), f16)
         keep += [e_buf, d_buf]
         for blk in P["blocks"]:
             inv, dw, pc = blk["inv"], blk["dw"], blk["pc"]
@@ -321,10 +323,16 @@ class LitePoseEngine(object):
             keep.append(out)
             if "wblk" in inv:
                 # the whole block in one kernel: the 6x-expanded tensor never reaches HBM
-                ops.append(_Op("block_s1", lib.lp_block_s1_f16,
-                               [cur.data_ptr(), inv["wblk"].data_ptr(), inv["bblk"].data_ptr(), dw["w"].data_ptr(),
-                                dw["b"].data_ptr(), pc["w"].data_ptr(), pc["b"].data_ptr(), 1 if blk["res"] else 0,
-                                out.data_ptr(), n, ch, cw_, inv["K"], dw["C"], pc["N"]]))
+                if blk["stride"] == 1:
+                    ops.append(_Op("block_s1", lib.lp_block_s1_f16,
+                                   [cur.data_ptr(), inv["wblk"].data_ptr(), inv["bblk"].data_ptr(), dw["w"].data_ptr(),
+                                    dw["b"].data_ptr(), pc["w"].data_ptr(), pc["b"].data_ptr(), 1 if blk["res"] else 0,
+                                    out.data_ptr(), n, ch, cw_, inv["K"], dw["C"], pc["N"]]))
+                else:
+                    ops.append(_Op("block_s2", lib.lp_block_s2_f16,
+                                   [cur.data_ptr(), inv["wblk"].data_ptr(), inv["bblk"].data_ptr(), dw["w"].data_ptr(),
+                                    dw["b"].data_ptr(), pc["w"].data_ptr(), pc["b"].data_ptr(), out.data_ptr(), n, ch,
+                                    cw_, inv["K"], dw["C"], pc["N"]]))
                 cur, ch, cw_ = out, oh, ow
                 if blk["last"]:
                     x_list.append((cur, ch, cw_))
