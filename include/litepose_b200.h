@@ -78,6 +78,8 @@ int lp_stem_conv3x3_s2(const void* x, int x_is_fp32, int flip_x, const void* w, 
  * fp16: row co = the 27 BN-folded taps of output channel co (k = c*9 + ky*3 + kx), zero padded; w_dw [9][32] tap-major;
  * w_pw_packed / b_pw_packed from lp_pw1x1_pack(K = 32, N = C0); out [N,H/2,W/2,C0] fp16 NHWC.  flip_x must be 0 or 1
  * (LP_ERR_BAD_ARG otherwise).  The two 32-channel half-resolution intermediates never reach HBM.
+ * An fp32 image is rounded to fp16 (round to nearest even) as it is loaded: the output for an fp32 x equals, bit for
+ * bit, the output for x converted to fp16.  (lp_stem_conv3x3_s2 does not round: it convolves the fp32 values.)
  * lp_stem_fused_supported: H even, W % 4 == 0, C0 % 8 == 0, C0 <= 32. */
 int lp_stem_fused_supported(int H, int W, int C0);
 int lp_stem_fused_f16(const void* x, int x_is_fp32, int flip_x, const void* w1_packed, const float* b1, const void* w_dw,

@@ -47,6 +47,39 @@ def _record(what, err, lim):
         pass
 
 
+def check_bound(got, ref, mag, k, what):
+    """got against the fp64 value ref of a K-term reduction, element by element: |got - ref| <= 2^-11 |ref| +
+    K 2^-22 mag + 2^-24, mag = the same reduction over absolute values.  The K 2^-22 mag term assumes Hopper's fp32
+    tensor-core accumulation loses at most a few bits per product (an assumption, not a measured figure); the worst
+    err / bound is recorded with _record."""
+    got = np.asarray(got, np.float64).reshape(ref.shape)
+    assert np.isfinite(got).all(), what
+    bound = 2.0 ** -11 * np.abs(ref) + k * 2.0 ** -22 * mag + 2.0 ** -24
+    ratio = np.abs(got - ref) / bound
+    worst = float(ratio.max())
+    _record("fp64 " + what, worst, 1.0)
+    assert worst <= 1.0, "%s: err/bound %.3f at %s" % (what, worst, np.unravel_index(ratio.argmax(), ratio.shape))
+
+
+def check_reduction(got, a, wt, bias, res, k, what, act=_lib.ACT_NONE):
+    """got [M, N] against act(a @ wt^T + bias) + res in fp64, element by element (check_bound)"""
+    a64, w64 = a.reshape(-1, k).astype(np.float64), wt.astype(np.float64)
+    ref = a64 @ w64.T
+    mag = np.abs(a64) @ np.abs(w64).T
+    if bias is not None:
+        ref += bias.astype(np.float64)
+        mag += np.abs(bias.astype(np.float64))
+    if act == _lib.ACT_RELU:
+        ref = np.maximum(ref, 0)
+    elif act == _lib.ACT_RELU6:
+        ref = np.clip(ref, 0, 6)
+    if res is not None:
+        r64 = res.reshape(ref.shape).astype(np.float64)
+        ref += r64
+        mag += np.abs(r64)
+    check_bound(got, ref, mag, k, what)
+
+
 def pack_pw(w, bias):
     lib = _lib.load()
     n, k = w.shape

@@ -3,14 +3,15 @@ lp_pw1x1_f16 (ReLU6) -> lp_dwconv_f16 (k7, stride 2, ReLU6, packed fp16) -> lp_p
 
 Both expand with one wgmma per K=16 slice and round (acc + bias) to fp16 before the ReLU6, both run the depthwise chain
 of dw_inner.cuh (stride 2 has no mirrored lanes), and both project over the same K=16 slices in channel order (four per
-64-channel K block, the slices past Ce adding exact zeros) with one rounding of acc + bias."""
+64-channel K block, the slices past Ce adding exact zeros) with one rounding of acc + bias.  At the LitePose shapes
+the fused output is also checked against fp64 over the emulated depthwise (dw_emul.dwconv) of the expansion."""
 import numpy as np
 import pytest
 import torch
 
 import dw_emul as de
 from litepose_b200 import _lib
-from gpu_util import pack_pw, stream
+from gpu_util import check_reduction, pack_pw, stream
 
 pytestmark = pytest.mark.gpu
 
@@ -105,6 +106,23 @@ def test_block_s2_equals_pw1x1_dwconv_pw1x1(n, h, w, cin, ce, co):
     lib.lp_set_dw_precision(-1)
     blk = _Block(n, h, w, cin, ce, co, cin * 5 + ce * 3 + co + h + w + n)
     assert_equal_values(blk.fused(), blk.chain(), "block_s2 n%d %dx%d cin%d ce%d co%d" % (n, h, w, cin, ce, co))
+
+
+@pytest.mark.parametrize("n,h,w,cin,ce,co", SHAPES[:3])
+def test_block_s2_projection_fp64_over_emulated_depthwise(n, h, w, cin, ce, co):
+    """the fused kernel's depthwise tied to the emulator directly, not only through lp_dwconv_f16: the projection of
+    the fused output checked element by element against fp64 over dw_emul.dwconv of the expansion (run by
+    lp_pw1x1_f16), at the LitePose-XS / S / M shapes"""
+    lib = _lib.load()
+    lib.lp_set_dw_precision(-1)
+    seed = cin * 5 + ce * 3 + co + h + w + n
+    blk = _Block(n, h, w, cin, ce, co, seed)
+    _, _, _, wd, bd, wp, bp = _inputs(n, h, w, cin, ce, co, seed)
+    e = _pw(blk.xd, blk.wek2, blk.bek2, n * h * w, cin, ce, de.ACT_RELU6)
+    torch.cuda.synchronize()
+    d = de.dwconv(e.cpu().numpy().reshape(n, h, w, ce), wd, bd, 7, 2, de.ACT_RELU6, 2)
+    check_reduction(blk.fused().reshape(-1, co), d, wp, bp, None, ce,
+                    "block_s2 n%d %dx%d cin%d ce%d co%d" % (n, h, w, cin, ce, co))
 
 
 def test_block_s2_repeated_launches_identical():

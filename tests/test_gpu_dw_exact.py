@@ -18,7 +18,7 @@ import torch
 
 import dw_emul as de
 from litepose_b200 import _lib
-from gpu_util import _record, pack_pw, stream
+from gpu_util import check_reduction, pack_pw, stream
 
 pytestmark = pytest.mark.gpu
 
@@ -279,31 +279,6 @@ def test_head_fused_equals_dwconv_then_head_pw_dual(n, h, w, c1, c2, co, fp32, d
 
 
 # ---------------------------------------------------------------- (d) tensor-core reductions against fp64
-def check_reduction(got, a, wt, bias, res, k, what, act=de.ACT_NONE):
-    """got [M, N] against act(a @ wt^T + bias) + res in fp64, element by element"""
-    a64, w64 = a.reshape(-1, k).astype(np.float64), wt.astype(np.float64)
-    ref = a64 @ w64.T
-    mag = np.abs(a64) @ np.abs(w64).T
-    if bias is not None:
-        ref += bias.astype(np.float64)
-        mag += np.abs(bias.astype(np.float64))
-    if act == de.ACT_RELU:
-        ref = np.maximum(ref, 0)
-    elif act == de.ACT_RELU6:
-        ref = np.clip(ref, 0, 6)
-    if res is not None:
-        r64 = res.reshape(ref.shape).astype(np.float64)
-        ref += r64
-        mag += np.abs(r64)
-    got = np.asarray(got, np.float64).reshape(ref.shape)
-    assert np.isfinite(got).all(), what
-    bound = 2.0 ** -11 * np.abs(ref) + k * 2.0 ** -22 * mag + 2.0 ** -24
-    ratio = np.abs(got - ref) / bound
-    worst = float(ratio.max())
-    _record("fp64 " + what, worst, 1.0)
-    assert worst <= 1.0, "%s: err/bound %.3f at %s" % (what, worst, np.unravel_index(ratio.argmax(), ratio.shape))
-
-
 DW7_PROJECT_FP64_SHAPES = [
     (2, 32, 32, 96, 16, True), (2, 16, 16, 144, 24, True), (2, 48, 32, 192, 32, True), (1, 20, 36, 224, 64, False),
     (2, 37, 45, 40, 64, True), (1, 32, 32, 720, 120, True), (1, 20, 40, 432, 72, False), (1, 16, 16, 960, 160, True),
