@@ -84,7 +84,6 @@ class LitePoseEngine(object):
         self.plans = {}
         self.arena_plans = collections.OrderedDict()    # LRU of plans whose buffers live in self.arenas
         self.arenas = {}                                # pass -> uint8 arena shared by every arena plan of that pass
-        self.use_graphs = False
 
     # ------------------------------------------------------------------ folded checkpoint ("next" row 4)
     # BN fold (reference fuse_bn.py:81-162) and kernel packing become a load-time no-op: the file holds exactly the
@@ -376,7 +375,7 @@ class LitePoseEngine(object):
                                [refined.data_ptr(), raw.data_ptr(), hd["dw_cat"].data_ptr(),
                                 hd["bdw_cat"].data_ptr(), hd["pw_cat"].data_ptr(), o.data_ptr(),
                                 1 if out_fp32 else 0, n, rh, rw, hd["C1"], hd["C2"], hd["Co"]]))
-        plan.update({"ops": ops, "outs": outs, "keep": keep, "graph": None, "static_in": None})
+        plan.update({"ops": ops, "outs": outs, "keep": keep})
         return plan
 
     def plan_for(self, n, h, w, in_dtype, out_fp32, flip=False, slot=0):
@@ -447,28 +446,8 @@ class LitePoseEngine(object):
         else:
             plan = self.plan_for(n, h, w, x.dtype, out_fp32, flip, slot)
         with torch.cuda.device(self.device):
-            stream = torch.cuda.current_stream().cuda_stream
-            if self.use_graphs and not arena:
-                g = plan["graph"]
-                if g is None:
-                    g = plan["graph"] = {}
-                key = 0
-                if plan["static_in"] is None:
-                    plan["static_in"] = torch.empty_like(x)
-                plan["static_in"].copy_(x)
-                if key not in g:
-                    plan["in_ptr"].value = plan["static_in"].data_ptr()
-                    plan["flip"].value = 1 if flip else 0
-                    self._launch_all(plan, stream)      # warm-up (also sets func attributes)
-                    torch.cuda.current_stream().synchronize()
-                    cg = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(cg):
-                        self._launch_all(plan, torch.cuda.current_stream().cuda_stream)
-                    g[key] = cg
-                g[key].replay()
-            else:
-                plan["in_ptr"].value = x.data_ptr()
-                plan["flip"].value = 1 if flip else 0
-                self._launch_all(plan, stream)
+            plan["in_ptr"].value = x.data_ptr()
+            plan["flip"].value = 1 if flip else 0
+            self._launch_all(plan, torch.cuda.current_stream().cuda_stream)
         outs = plan["outs"]
         return [o.clone() for o in outs] if clone else list(outs)

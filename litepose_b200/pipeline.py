@@ -147,16 +147,21 @@ class LitePosePipeline(object):
         # never clipped: step() fetches the full result from the parser's buffers (capacity J*K persons) in a second
         # copy, and unpack() raises if it is handed an overflowing payload without that second copy.
         self.keep = min(int(keep), self.parser.pcap)
+        J = p.num_joints
         if grouping == "fast":
             from .fast_utils.group import Params as FastParams
             fp = FastParams(cfg)
-            J = p.num_joints
             # the demo's parser hands joint_order to assign(), which reads the first C entries: the entries that name no
             # plane are dropped, as fast_utils.group.HeatmapParser._joint_order does
             self.fast = {"M": int(fp.max_num_people), "thr": float(fp.detection_threshold), "win": int(fp.window_size),
                          "tag_thr": float(fp.tag_threshold),
                          "jo": torch.tensor([j for j in fp.joint_order if j < J][:J], dtype=torch.int32,
                                             device=self.device)}
+        # packed payload per image: ae = ``keep`` persons x J x (x, y, val, T tags) | their scores | person count;
+        # fast = every person (M <= 32) x J x (x, y, val, tag) | person count | KM status
+        self.T = 2 if self.flip else 1
+        self.row = J * (3 + self.T)
+        self.width = self.fast["M"] * J * 4 + 2 if grouping == "fast" else self.keep * self.row + self.keep + 1
         self._state = {}
         self._async = None                # submit()/collect() slots
         self._final = None                # per-image inverse affines of get_final_preds (host, [N,6] float64)
@@ -221,16 +226,15 @@ class LitePosePipeline(object):
             for c, s in zip(*self._final)]).reshape(-1, 6))
 
     # -- device step (everything between the H2D copy and the D2H copy) -------------
-    def _network_part(self, st, x, slot=0, arena=False):
+    def _network_part(self, side, x, slot=0, arena=False):
         """Both network passes -> ([o0, o1], [f0, f1]) in the engine's buffer set ``slot`` (``arena``: in the engine's
-        shared arena plans, see LitePoseEngine.arena_plan_for)."""
+        shared arena plans, see LitePoseEngine.arena_plan_for); the mirrored pass runs on the stream ``side``."""
         eng = self.engine
         if not self.flip:
             return eng.run(x, flip=False, out_fp32=True, clone=False, slot=slot, arena=arena), None
         # the plain and the mirrored pass are independent until the glue: fork onto a side stream so that one pass'
         # kernels fill the launch gaps and tails of the other (each pass has its own plan buffers)
         main = torch.cuda.current_stream()
-        side = st["side"]
         side.wait_stream(main)
         with torch.cuda.stream(side):
             f = eng.run(x, flip=True, out_fp32=True, clone=False, slot=slot, arena=arena)
@@ -238,49 +242,92 @@ class LitePosePipeline(object):
         main.wait_stream(side)
         return o, f
 
-    def _glue_part(self, st, o, f, det, tag):
-        """Fused glue (+ the benchmark's planted persons) on the four model outputs -> det / tag of this step."""
-        J = self.params.num_joints
-        o0, o1 = o[0], o[1]
-        n, _, h, w = o0.shape
-        Hd, Wd = det.shape[2], det.shape[3]
+    def _glue(self, o, f, det, tag, plant, i=0):
+        """Glue launch of scale ``i`` of self.scales (largest first) on that scale's model outputs, into det / tag:
+        lp_glue_f32 for the canonical single-scale layout, else lp_glue_scale_f32 (see step_device_multiscale).  After
+        the last scale, the benchmark's planted persons: ``plant`` is one PlantedCrowd, a list with one (or None) per
+        image, or None."""
+        n, J, Hd, Wd = det.shape[0], self.params.num_joints, det.shape[2], det.shape[3]
+        h, w = o[0].shape[2], o[0].shape[3]
         fl = 1 if self.flip else 0
         f0, f1 = (f[0].data_ptr(), f[1].data_ptr()) if self.flip else (None, None)
+        last = i == len(self.scales) - 1
         stream = torch.cuda.current_stream().cuda_stream
-        if self.canonical:
-            _lib.check(self.lib.lp_glue_f32(o0.data_ptr(), o1.data_ptr(), f0, f1, self.fidx.data_ptr(), n, J, h, w, fl, Hd,
-                                            Wd, det.data_ptr(), tag.data_ptr(), stream), "lp_glue_f32")
+        if self.canonical and len(self.scales) == 1:
+            _lib.check(self.lib.lp_glue_f32(o[0].data_ptr(), o[1].data_ptr(), f0, f1, self.fidx.data_ptr(), n, J, h, w,
+                                            fl, Hd, Wd, det.data_ptr(), tag.data_ptr(), stream), "lp_glue_f32")
         else:
-            _lib.check(self.lib.lp_glue_scale_f32(o0.data_ptr(), o1.data_ptr(), f0, f1, self.fidx.data_ptr(), n, J,
-                                                  self.model_joints, 1 if self.tag_shared else 0, h, w, fl, Hd, Wd, 0, 1.0,
-                                                  det.data_ptr(), tag.data_ptr(), stream), "lp_glue_scale_f32")
-        if st["plant"] is not None:
-            st["plant"].apply(det, tag)
+            _lib.check(self.lib.lp_glue_scale_f32(
+                o[0].data_ptr(), o[1].data_ptr(), f0, f1, self.fidx.data_ptr(), n, J, self.model_joints,
+                1 if self.tag_shared else 0, h, w, fl, Hd, Wd, 1 if i > 0 else 0,
+                float(len(self.scales)) if last else 1.0, det.data_ptr(),
+                tag.data_ptr() if self.scales[i] == 1.0 else None, stream), "lp_glue_scale_f32")
+        if not last:
+            return
+        if isinstance(plant, list):
+            for k, p in enumerate(plant):
+                if p is not None:
+                    p.apply(det[k:k + 1], tag[k:k + 1])
+        elif plant is not None:
+            plant.apply(det, tag)
 
-    def _forward_part(self, st, x, det, tag):
-        """Both network passes + fused glue (+ the benchmark's planted persons) -> det / tag of this step."""
-        o, f = self._network_part(st, x)
-        self._glue_part(st, o, f, det, tag)
+    def _forward(self, xs, det, tag, side, plant, arena=False):
+        """``xs``: {scale: frames [N,3,Hs,Ws] on the device}, or the frames alone for a single-scale cfg.  Per scale,
+        largest first: both network passes and the glue launch into det / tag (+ the planted persons, see _glue)."""
+        if not isinstance(xs, dict):
+            xs = {1.0: xs}
+        for i, s in enumerate(self.scales):
+            o, f = self._network_part(side, xs[s], arena=arena)
+            self._glue(o, f, det, tag, plant, i)
+
+    def _parse(self, det, tag, packed, trans, fb=None, ragged=None):
+        """The grouping mode's device parser, get_final_preds (``trans``: device pointer to [N,6] float64 matrices, or
+        None) and payload pack on det / tag -> ``packed``.  Uniform maps: det [N,J,H,W], tag [N,1|J,H,W,T]; ragged
+        arena: ``ragged`` = (hw [N,2] host int32, device pointer to the lp_map_desc_t of the maps).  ``fb``: the fast
+        grouping's buffers (_fast_buffers).  Returns the ae parser's own buffers (ans, num, scores; capacity J*K
+        persons, valid until its next run) for fetch_overflow; None with grouping="fast"."""
+        J, T = self.params.num_joints, self.T
+        hw, desc = ragged if ragged is not None else (None, None)
+        n = det.shape[0] if ragged is None else len(hw)
+        s = torch.cuda.current_stream().cuda_stream
+        full = None
+        if self.grouping == "fast":
+            # the demo's parser where the glue left the maps: zero ans, find peaks (tag channel 0 read in place), KM
+            # assignment
+            f, M = self.fast, self.fast["M"]
+            ans, num = fb["ans"], fb["num"]
+            # lp_assign_f32 writes only the entries it assigns: without this the rows of the previous step would remain
+            ans.zero_()
+            H, W = (det.shape[2], det.shape[3]) if ragged is None else (0, 0)
+            _lib.check(self.lib.lp_find_peaks_maps_f32(
+                det.data_ptr(), tag.data_ptr(), n, H, W, None if hw is None else hw.ctypes.data, desc, J, T,
+                1 if self.tag_shared else J, M, f["thr"], f["win"], fb["count"].data_ptr(), fb["val"].data_ptr(),
+                fb["tag"].data_ptr(), fb["ind"].data_ptr(), s), "lp_find_peaks_maps_f32")
+            _lib.check(self.lib.lp_assign_f32(fb["count"].data_ptr(), fb["val"].data_ptr(), fb["tag"].data_ptr(),
+                                              fb["ind"].data_ptr(), f["jo"].data_ptr(), n, J, M, f["tag_thr"],
+                                              num.data_ptr(), ans.data_ptr(), fb["status"].data_ptr(), s), "lp_assign_f32")
+        elif ragged is not None:
+            ans, num, scores = full = self.parser.run_ragged(det, tag, hw, desc, T, self.adjust, self.refine)
+        else:
+            if self.tag_shared:
+                # MODEL.TAG_PER_JOINT off: the one tag map serves every joint (group.py:150-152); the parser kernels
+                # index [N,J,H,W,T], so the map is tiled here (one strided copy; not the shipped configuration)
+                tag = tag.expand(-1, J, -1, -1, -1).contiguous()
+            ans, num, scores = full = self.parser.run(det, tag, self.adjust, self.refine)
+        if trans is not None:
+            _lib.check(self.lib.lp_transform_preds_f32(ans.data_ptr(), num.data_ptr(), trans, n, ans.shape[1],
+                                                       ans.shape[2], ans.shape[3], s), "lp_transform_preds_f32")
+        if self.grouping == "fast":
+            _lib.check(self.lib.lp_pack_fast_payload_f32(ans.data_ptr(), num.data_ptr(), fb["status"].data_ptr(), n, M,
+                                                         J, packed.data_ptr(), s), "lp_pack_fast_payload_f32")
+        else:
+            _lib.check(self.lib.lp_pack_payload_f32(ans.data_ptr(), num.data_ptr(), scores.data_ptr(), n, ans.shape[1],
+                                                    self.row, self.keep, packed.data_ptr(), s), "lp_pack_payload_f32")
+        return full
 
     def _parser_part(self, st, det, tag, packed):
-        """Device parser (+ get_final_preds) on det / tag -> packed fixed-size payload."""
-        n = det.shape[0]
-        if self.grouping == "fast":
-            return self._fast_parser_part(st, det, tag, packed)
-        if self.tag_shared:
-            # MODEL.TAG_PER_JOINT off: the one tag map serves every joint (group.py:150-152); the parser kernels index
-            # [N,J,H,W,T], so the map is tiled here (one strided copy; not the shipped configuration)
-            tag = tag.expand(-1, det.shape[1], -1, -1, -1).contiguous()
-        ans, num, scores = self.parser.run(det, tag, self.adjust, self.refine)
-        if st["trans"] is not None:
-            _lib.check(self.lib.lp_transform_preds_f32(ans.data_ptr(), num.data_ptr(), st["trans"].data_ptr(), n,
-                                                       ans.shape[1], ans.shape[2], ans.shape[3],
-                                                       torch.cuda.current_stream().cuda_stream), "lp_transform_preds_f32")
-        st["full"] = (ans, num, scores)       # parser-owned buffers (capacity J*K persons), valid until the next step
-        _lib.check(self.lib.lp_pack_payload_f32(ans.data_ptr(), num.data_ptr(), scores.data_ptr(), n, ans.shape[1],
-                                                st["row"], self.keep, packed.data_ptr(),
-                                                torch.cuda.current_stream().cuda_stream), "lp_pack_payload_f32")
-        return packed
+        """_parse on maps of the uniform-size state ``st`` -> ``packed``; the ae parser's buffers stay in st["full"]."""
+        st["full"] = self._parse(det, tag, packed, None if st["trans"] is None else st["trans"].data_ptr(), st["fast"])
 
     def _fast_buffers(self, n, J, alloc=None):
         """Peaks, persons and status of the fast grouping for n images; ``alloc(name, shape, dtype)`` (default: new
@@ -292,49 +339,47 @@ class LitePosePipeline(object):
                 "ans": ((n, M, J, 4), f32), "num": ((n,), i32), "status": ((n,), i32)}
         return {k: alloc(k, shape, dt) for k, (shape, dt) in spec.items()}
 
-    def _fast_parse(self, b, det, tag, n, J, T, tag_planes, hw, desc, trans, packed):
-        """The demo's parser on det / tag where the glue left them: zero ans, find peaks (tag channel 0 read in place),
-        KM assignment, get_final_preds (``trans``: device [N,6] float64 or None), pack.  Uniform maps: ``hw`` / ``desc``
-        None, det [N,J,H,W]; ragged arena: ``hw`` [N,2] host int32 and ``desc`` the device lp_map_desc_t pointer."""
-        f, M = self.fast, self.fast["M"]
-        s = torch.cuda.current_stream().cuda_stream
-        ans = b["ans"]
-        # lp_assign_f32 writes only the entries it assigns: without this the rows of the previous step would remain
-        ans.zero_()
-        H, W = (det.shape[2], det.shape[3]) if desc is None else (0, 0)
-        _lib.check(self.lib.lp_find_peaks_maps_f32(
-            det.data_ptr(), tag.data_ptr(), n, H, W, None if hw is None else hw.ctypes.data, desc, J, T, tag_planes, M,
-            f["thr"], f["win"], b["count"].data_ptr(), b["val"].data_ptr(), b["tag"].data_ptr(), b["ind"].data_ptr(), s),
-            "lp_find_peaks_maps_f32")
-        _lib.check(self.lib.lp_assign_f32(b["count"].data_ptr(), b["val"].data_ptr(), b["tag"].data_ptr(),
-                                          b["ind"].data_ptr(), f["jo"].data_ptr(), n, J, M, f["tag_thr"],
-                                          b["num"].data_ptr(), ans.data_ptr(), b["status"].data_ptr(), s), "lp_assign_f32")
-        if trans is not None:
-            _lib.check(self.lib.lp_transform_preds_f32(ans.data_ptr(), b["num"].data_ptr(), trans, n, M, J, 4, s),
-                       "lp_transform_preds_f32")
-        _lib.check(self.lib.lp_pack_fast_payload_f32(ans.data_ptr(), b["num"].data_ptr(), b["status"].data_ptr(), n, M,
-                                                     J, packed.data_ptr(), s), "lp_pack_fast_payload_f32")
-        return packed
-
-    def _fast_parser_part(self, st, det, tag, packed):
-        n, J = det.shape[0], det.shape[1]
-        trans = st["trans"].data_ptr() if st["trans"] is not None else None
-        return self._fast_parse(st["fast"], det, tag, n, J, tag.shape[4], tag.shape[1], None, None, trans, packed)
-
     def unpack_fast(self, host):
         """Fast-grouping payload (host) -> list over images of (ans ndarray [P,J,4], P); see unpack_fast_payload."""
         return unpack_fast_payload(host, self.fast["M"], self.params.num_joints)
 
-    def _result(self, st, host):
-        """Host payload of a blocking call -> per-image results of the pipeline's grouping mode."""
+    def _decode(self, host, st=None):
+        """Host payload -> per-image results of the pipeline's grouping mode.  fast: raises on a KM status 1; ae: the
+        images past ``keep`` are read from the parser's buffers of the step ``st`` that produced ``host``
+        (fetch_overflow), and raise without it."""
         if self.grouping == "fast":
             return self.unpack_fast(host)
-        return self.unpack(host, st["row"], st["T"], self.fetch_overflow(st, host))
+        return self.unpack(host, self.row, self.T, None if st is None else self.fetch_overflow(st, host))
 
-    # -- device step (everything between the H2D copy and the D2H copy) -------------
-    def _device_step(self, st, x):
-        self._forward_part(st, x, st["det"], st["tag"])
-        return self._parser_part(st, st["det"], st["tag"], st["packed"])
+    def _fetch(self, st):
+        """Blocking result of a step: D2H copy of st["packed"] into the pinned st["host"], synchronise, _decode."""
+        st["host"].copy_(st["packed"], non_blocking=True)
+        torch.cuda.current_stream().synchronize()
+        return self._decode(st["host"], st)
+
+    def _forward_part(self, st, xs, det, tag):
+        """_forward on the side stream and plant hook of the uniform-size state ``st``."""
+        self._forward(xs, det, tag, st["side"], st["plant"])
+
+    def _device_step(self, st, xs):
+        """Network passes, glue and parser of one step on ``xs`` (see _forward) into the buffers of ``st``."""
+        self._forward_part(st, xs, st["det"], st["tag"])
+        self._parser_part(st, st["det"], st["tag"], st["packed"])
+
+    @staticmethod
+    def _capture(*parts):
+        """One CUDA graph per callable of ``parts``, captured in order after an eager run of them all (which builds the
+        engine's plans and sets the kernels' function attributes) and a synchronise."""
+        for part in parts:
+            part()
+        torch.cuda.synchronize()
+        graphs = []
+        for part in parts:
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                part()
+            graphs.append(g)
+        return graphs
 
     def step_device_overlapped(self, x_dev, plant=None):
         """Throughput form of step_device: the network passes of this step run on the current stream while the glue and
@@ -365,22 +410,19 @@ class LitePosePipeline(object):
             for ev in ov["P_done"]:
                 if ev is not None:
                     main.wait_event(ev)
-            self.engine.use_graphs = False
-            o, f = self._network_part(st, st["x"], slot=b)       # warm-up: builds plans, sets attributes
-            self._glue_part(st, o, f, ov["det"][b], ov["tag"][b])
-            self._parser_part(st, ov["det"][b], ov["tag"][b], ov["packed"][b])
-            torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                o, f = self._network_part(st, st["x"], slot=b)
-            ov["gF"][b] = g
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
+            det, tag, packed = ov["det"][b], ov["tag"][b], ov["packed"][b]
+            of = []
+
+            def network():
+                of[:] = self._network_part(st["side"], st["x"], slot=b)
+
+            def glue_parse():
                 # the glue writes 1.4 GB at the HBM write roofline: on the second stream it overlaps the FMA-bound network
                 # passes of the next step (which write the other buffer set of the engine)
-                self._glue_part(st, o, f, ov["det"][b], ov["tag"][b])
-                self._parser_part(st, ov["det"][b], ov["tag"][b], ov["packed"][b])
-            ov["gP"][b] = g
+                self._glue(of[0], of[1], det, tag, st["plant"])
+                self._parser_part(st, det, tag, packed)
+
+            ov["gF"][b], ov["gP"][b] = self._capture(network, glue_parse)
         ov["gF"][b].replay()
         f_done = torch.cuda.Event()
         f_done.record(main)
@@ -403,21 +445,16 @@ class LitePosePipeline(object):
         st = self._state.get(key)
         if st is None:
             J = self.params.num_joints
-            T = 2 if self.flip else 1
             Hd, Wd = det_hw if det_hw is not None else ((s_h, s_w) if self.project else (s_h // 2, s_w // 2))
             dev = self.device
-            row = J * (3 + T)
-            width = self.keep * row + self.keep + 1
-            if self.grouping == "fast":            # every person (M <= 32) x J x (x, y, val, tag) | count | KM status
-                width = self.fast["M"] * J * 4 + 2
             st = {
                 "x": torch.empty((n, 3, s_h, s_w), dtype=dtype, device=dev),
                 "side": torch.cuda.Stream(device=dev),
                 "det": torch.empty((n, J, Hd, Wd), dtype=torch.float32, device=dev),
-                "tag": torch.empty((n, 1 if self.tag_shared else J, Hd, Wd, T), dtype=torch.float32, device=dev),
-                "packed": torch.zeros((n, width), dtype=torch.float32, device=dev),
-                "host": torch.empty((n, width), dtype=torch.float32).pin_memory(),
-                "row": row, "T": T, "graph": None, "plant": plant, "trans": None, "full": None, "ov": None,
+                "tag": torch.empty((n, 1 if self.tag_shared else J, Hd, Wd, self.T), dtype=torch.float32, device=dev),
+                "packed": torch.zeros((n, self.width), dtype=torch.float32, device=dev),
+                "host": torch.empty((n, self.width), dtype=torch.float32).pin_memory(),
+                "row": self.row, "T": self.T, "graph": None, "plant": plant, "trans": None, "full": None, "ov": None,
                 "fast": self._fast_buffers(n, J) if self.grouping == "fast" else None,
             }
             if self._final is not None:
@@ -442,7 +479,9 @@ class LitePosePipeline(object):
         [N, keep*J*(3+T) + keep + 1] (keypoints, scores, person count); with grouping="fast" [N, M*J*4 + 2] (every
         person's keypoints, person count, KM status: unpack_fast_payload)."""
         n, _, s_h, s_w = x_dev.shape
-        st = self._get_state(n, s_h, s_w, x_dev.dtype, plant)
+        # the state of the last step_device / step_device_multiscale call: its det / tag / packed stay readable there
+        # until the next call
+        st = self._last_state = self._get_state(n, s_h, s_w, x_dev.dtype, plant)
         ov = st.get("ov")
         if ov is not None:
             # det / tag / packed are shared with buffer set 0 of the overlapped form: an overlapped step that is still
@@ -451,28 +490,18 @@ class LitePosePipeline(object):
                 if ev is not None:
                     torch.cuda.current_stream().wait_event(ev)
         if not self.use_graphs:
-            return self._device_step(st, x_dev)
+            self._device_step(st, x_dev)
+            return st["packed"]
         st["x"].copy_(x_dev, non_blocking=True)
         if st["graph"] is None:
-            self.engine.use_graphs = False
-            self._device_step(st, st["x"])          # warm-up: builds plans, sets function attributes
-            torch.cuda.current_stream().synchronize()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self._device_step(st, st["x"])
-            st["graph"] = g
+            st["graph"], = self._capture(lambda: self._device_step(st, st["x"]))
         st["graph"].replay()
         return st["packed"]
 
     def step(self, frames_pinned, plant=None):
         """Public end-to-end call: pinned host frames in, host result out (blocking)."""
-        x = frames_pinned.to(self.device, non_blocking=True)
-        packed = self.step_device(x, plant)
-        n = packed.shape[0]
-        st = self._get_state(n, x.shape[2], x.shape[3], x.dtype, plant)
-        st["host"].copy_(packed, non_blocking=True)
-        torch.cuda.current_stream().synchronize()
-        return self._result(st, st["host"])
+        self.step_device(frames_pinned.to(self.device, non_blocking=True), plant)
+        return self._fetch(self._last_state)
 
     # -- multi-scale test (TEST.SCALE_FACTOR with several entries; reference valid.py:198-229) ----------------------------
     def step_device_multiscale(self, xs, plant=None):
@@ -488,51 +517,23 @@ class LitePosePipeline(object):
         missing = [s for s in scales if s not in xs]
         if missing:
             raise ValueError("step_device_multiscale: no frames for scale(s) %r" % (missing,))
-        x1 = xs[1.0]
+        x1, big = xs[1.0], xs[scales[0]]
         n = x1.shape[0]
-        big = xs[scales[0]]
-        det_hw = (x1.shape[2], x1.shape[3]) if self.project else (big.shape[2] // 2, big.shape[3] // 2)
-        st = self._get_state(n, x1.shape[2], x1.shape[3], x1.dtype, plant, det_hw=det_hw)
-        det, tag = st["det"], st["tag"]
-        self.engine.use_graphs = False
-        self._multiscale_part(st, xs, det, tag, det_hw)
-        if st["plant"] is not None:
-            st["plant"].apply(det, tag)
-        return self._parser_part(st, det, tag, st["packed"])
-
-    def _multiscale_part(self, st, xs, det, tag, det_hw, arena=False):
-        """Per scale, largest first: both network passes and one lp_glue_scale_f32 launch accumulating into det (the
-        tags from the scale-1 pass); the last launch divides by the number of scales."""
-        scales = self.scales
-        n = det.shape[0]
-        J = self.params.num_joints
-        stream = torch.cuda.current_stream().cuda_stream
-        for i, s in enumerate(scales):
+        for s in scales:
             x = xs[s]
             if x.shape[0] != n or x.shape[2] % 64 or x.shape[3] % 64:
                 raise ValueError("step_device_multiscale: scale %r frames %r (batch %d, sides multiples of 64 expected)"
                                  % (s, tuple(x.shape), n))
-            o, f = self._network_part(st, x, arena=arena)
-            _, _, h, w = o[0].shape
-            _lib.check(self.lib.lp_glue_scale_f32(
-                o[0].data_ptr(), o[1].data_ptr(), f[0].data_ptr() if self.flip else None,
-                f[1].data_ptr() if self.flip else None, self.fidx.data_ptr(), n, J, self.model_joints,
-                1 if self.tag_shared else 0, h, w, 1 if self.flip else 0, det_hw[0], det_hw[1], 1 if i > 0 else 0,
-                float(len(scales)) if i == len(scales) - 1 else 1.0,
-                det.data_ptr(), tag.data_ptr() if s == 1.0 else None, stream), "lp_glue_scale_f32")
+        det_hw = (x1.shape[2], x1.shape[3]) if self.project else (big.shape[2] // 2, big.shape[3] // 2)
+        st = self._last_state = self._get_state(n, x1.shape[2], x1.shape[3], x1.dtype, plant, det_hw=det_hw)
+        self._device_step(st, xs)
+        return st["packed"]
 
     def step_multiscale(self, frames, plant=None):
         """Public blocking call of the multi-scale test: {scale: pinned host frames} in, host result out (the list
         over images of (ans [P,J,3+T], scores, P), as step())."""
-        xs = {float(s): f.to(self.device, non_blocking=True) for s, f in frames.items()}
-        packed = self.step_device_multiscale(xs, plant)
-        x1 = xs[1.0]
-        big = xs[self.scales[0]]
-        det_hw = (x1.shape[2], x1.shape[3]) if self.project else (big.shape[2] // 2, big.shape[3] // 2)
-        st = self._get_state(x1.shape[0], x1.shape[2], x1.shape[3], x1.dtype, plant, det_hw=det_hw)
-        st["host"].copy_(packed, non_blocking=True)
-        torch.cuda.current_stream().synchronize()
-        return self._result(st, st["host"])
+        self.step_device_multiscale({float(s): f.to(self.device, non_blocking=True) for s, f in frames.items()}, plant)
+        return self._fetch(self._last_state)
 
     def infer_images(self, images, mean=(0.485, 0.456, 0.406), std=(0.229, 0.224, 0.225), half=True, plant=None):
         """The body of the reference's evaluation loop (valid.py:198-233) for a batch of equally sized uint8 images
@@ -561,19 +562,11 @@ class LitePosePipeline(object):
         prev = self._final                     # a caller's own set_final_preds() setting is put back afterwards
         self.set_final_preds([center] * n, [scale] * n)
         try:
-            x1 = xs[1.0]
             if len(self.scales) == 1:
-                packed = self.step_device(x1, plant)
-                det_hw = None
+                self.step_device(xs[1.0], plant)
             else:
-                packed = self.step_device_multiscale(xs, plant)
-                big = xs[self.scales[0]]
-                det_hw = (x1.shape[2], x1.shape[3]) if self.project else (big.shape[2] // 2, big.shape[3] // 2)
-            st = self._get_state(n, x1.shape[2], x1.shape[3], x1.dtype, plant, det_hw=det_hw)
-            self._last_state = st                 # det / tag of this call stay readable there until the next call
-            st["host"].copy_(packed, non_blocking=True)
-            torch.cuda.current_stream().synchronize()
-            return self._result(st, st["host"])
+                self.step_device_multiscale(xs, plant)
+            return self._fetch(self._last_state)
         finally:
             if prev is None:
                 self.set_final_preds(None)
@@ -608,15 +601,12 @@ class LitePosePipeline(object):
         n = len(shapes)
         if plant is not None and len(plant) != n:
             raise ValueError("infer_images: %d plant entries for %d images" % (len(plant), n))
-        J = self.params.num_joints
-        T = 2 if self.flip else 1
+        J, T = self.params.num_joints, self.T
         mp = MixedPlan(shapes, self.scales, int(self.cfg.DATASET.INPUT_SIZE), self.project, J, T)
         if not hasattr(self, "_mixed_bufs"):
             self._mixed_bufs = {}
             self._mixed_side = torch.cuda.Stream(device=self.device)
-        dev = self.device
         in_dtype = torch.float16 if half else torch.float32
-        main = torch.cuda.current_stream()
         # (1) one pinned staging buffer: the images (arena order) followed by the descriptors and final-pred matrices
         descs = [mp.warp_desc(s).view(np.uint8) for s in self.scales]
         mdesc = mp.map_desc().view(np.uint8)
@@ -646,7 +636,7 @@ class LitePosePipeline(object):
         # (2) per scale one ragged warp + ToTensor + Normalize into the scale's input arena
         mean_a, std_a = np.asarray(mean, np.float32), np.asarray(std, np.float32)
         xs_arena = {}
-        stream = main.cuda_stream
+        stream = torch.cuda.current_stream().cuda_stream
         for k, s in enumerate(self.scales):
             xa = self._grow("x%d" % k, int(mp.in_off[s][-1]), in_dtype)
             mh, mw = mp.max_in_hw(s)
@@ -657,7 +647,6 @@ class LitePosePipeline(object):
         # (3) per size group: the network passes + glue on the existing kernels, into the group's arena slice
         det_a = self._grow("det", int(mp.det_off[-1]), torch.float32)
         tag_a = self._grow("tag", int(mp.tag_off[-1]), torch.float32)
-        self.engine.use_graphs = False
         specs = []
         for g in mp.groups:
             for s in self.scales:
@@ -666,7 +655,6 @@ class LitePosePipeline(object):
                 if self.flip:
                     specs.append((g.n, hs, ws, in_dtype, True, True))
         self.engine.reserve_arena(specs)
-        st = {"side": self._mixed_side, "plant": None}
         for g in mp.groups:
             p0, p1 = g.start, g.start + g.n
             hd, wd = g.det_hw
@@ -676,48 +664,23 @@ class LitePosePipeline(object):
                 if self.tag_shared else tag_full
             xs = {s: xs_arena[s][int(mp.in_off[s][p0]):int(mp.in_off[s][p1])].view(g.n, 3, *g.in_hw[s])
                   for s in self.scales}
-            if len(self.scales) == 1:
-                o, f = self._network_part(st, xs[1.0], arena=True)
-                self._glue_part(st, o, f, det, tag)
-            else:
-                self._multiscale_part(st, xs, det, tag, g.det_hw, arena=True)
-            if plant is not None:
-                for k, i in enumerate(g.images):
-                    if plant[i] is not None:
-                        plant[i].apply(det[k:k + 1], tag[k:k + 1])
+            self._forward(xs, det, tag, self._mixed_side, None if plant is None else [plant[i] for i in g.images],
+                          arena=True)
             if self.tag_shared and self.grouping == "fast":
                 tag_full[:, :1].copy_(tag)          # the peak finder reads the shared map as plane 0 of the image's block
             elif self.tag_shared:
                 tag_full.copy_(tag.expand(-1, J, -1, -1, -1))
         # (4) once per batch: ragged parser, get_final_preds, payload, D2H
         hw = np.ascontiguousarray(mp.det_hw, np.int32)
+        fb = None
         if self.grouping == "fast":
-            M = self.fast["M"]
-            b = self._fast_buffers(n, J, lambda k, shape, dt: self._grow("fast_" + k, int(np.prod(shape)), dt).view(shape))
-            width = M * J * 4 + 2
-            packed = self._grow("packed", n * width, torch.float32).view(n, width)
-            self._fast_parse(b, det_a, tag_a, n, J, T, 1 if self.tag_shared else J, hw, d.data_ptr() + offs[-2],
-                             d.data_ptr() + offs[-1], packed)
-            out_h = self._grow("host", n * width, torch.float32, pinned=True).view(n, width)
-            out_h.copy_(packed, non_blocking=True)
-            main.synchronize()
-            res = self.unpack_fast(out_h)
-            self._last_mixed = {"plan": mp, "det": det_a, "tag": tag_a, "inputs": xs_arena}
-            return [res[int(p)] for p in mp.pos]
-        ans, num, scores = self.parser.run_ragged(det_a, tag_a, hw, d[offs[-2]:].data_ptr(), T, self.adjust, self.refine)
-        pcap = ans.shape[1]
-        _lib.check(self.lib.lp_transform_preds_f32(ans.data_ptr(), num.data_ptr(), d.data_ptr() + offs[-1], n, pcap, J,
-                                                   ans.shape[3], stream), "lp_transform_preds_f32")
-        row = J * (3 + T)
-        width = self.keep * row + self.keep + 1
+            fb = self._fast_buffers(n, J, lambda k, shape, dt: self._grow("fast_" + k, int(np.prod(shape)), dt).view(shape))
+        width = self.width
         packed = self._grow("packed", n * width, torch.float32).view(n, width)
-        _lib.check(self.lib.lp_pack_payload_f32(ans.data_ptr(), num.data_ptr(), scores.data_ptr(), n, pcap, row,
-                                                self.keep, packed.data_ptr(), stream), "lp_pack_payload_f32")
-        out_h = self._grow("host", n * width, torch.float32, pinned=True).view(n, width)
-        out_h.copy_(packed, non_blocking=True)
-        main.synchronize()
-        res = self.unpack(out_h, row, T, self.fetch_overflow({"full": (ans, num, scores)}, out_h))
-        self._last_mixed = {"plan": mp, "det": det_a, "tag": tag_a, "inputs": xs_arena}
+        full = self._parse(det_a, tag_a, packed, d.data_ptr() + offs[-1], fb, (hw, d.data_ptr() + offs[-2]))
+        self._last_mixed = {"plan": mp, "det": det_a, "tag": tag_a, "inputs": xs_arena, "packed": packed, "full": full,
+                            "host": self._grow("host", n * width, torch.float32, pinned=True).view(n, width)}
+        res = self._fetch(self._last_mixed)
         return [res[int(p)] for p in mp.pos]
 
     # -- asynchronous end-to-end API: two steps in flight -----------------------------------------
@@ -739,8 +702,7 @@ class LitePosePipeline(object):
                                    "shape, dtype or group")
             world = dist.get_world_size(group) if group is not None else 1
             rank = dist.get_rank(group) if group is not None else 0
-            st = self._get_state(n, s_h, s_w, frames_pinned.dtype, plant)
-            width = st["packed"].shape[1]
+            width = self.width
             slots = []
             for _ in range(2):
                 sl = {"x": torch.empty((n, 3, s_h, s_w), dtype=frames_pinned.dtype, device=self.device),
@@ -752,7 +714,7 @@ class LitePosePipeline(object):
                 slots.append(sl)
             a = self._async = {"key": (n, s_h, s_w, frames_pinned.dtype, id(group)), "slots": slots, "next": 0,
                                "copy": torch.cuda.Stream(device=self.device), "res": torch.cuda.Stream(device=self.device),
-                               "world": world, "rank": rank, "dst": dst, "group": group, "row": st["row"], "T": st["T"]}
+                               "world": world, "rank": rank, "dst": dst, "group": group}
         i = a["next"]
         sl = a["slots"][i]
         if sl["busy"]:
@@ -775,10 +737,10 @@ class LitePosePipeline(object):
         with torch.cuda.stream(a["res"]):
             a["res"].wait_event(parsed)
             sl["out"].copy_(packed, non_blocking=True)
-            st_ = self._get_state(n, s_h, s_w, frames_pinned.dtype, plant)
+            st = self._get_state(n, s_h, s_w, frames_pinned.dtype, plant)
             done = torch.cuda.Event()
             done.record(a["res"])
-            st_["ov"]["consumer_done"][st_["ov_last"]] = done
+            st["ov"]["consumer_done"][st["ov_last"]] = done
             if a["world"] > 1:
                 glist = list(sl["all"].unbind(0)) if a["rank"] == a["dst"] else None
                 dist.gather(sl["out"], glist, dst=a["dst"], group=group)
@@ -803,15 +765,15 @@ class LitePosePipeline(object):
         sl["busy"] = False
         if a["world"] > 1 and a["rank"] != a["dst"]:
             return None
-        if self.grouping == "fast":
-            res = [self.unpack_fast(sl["host"][r]) for r in range(sl["host"].shape[0])]      # raises on a KM status 1
-            return res if unpack else sl["host"]
-        if float(sl["host"][:, :, -1].max()) > self.keep:
-            raise _lib.LitePoseError("an image holds more persons than the packed payload carries (%d): use step() or "
-                                     "a larger keep" % self.keep)
-        if not unpack:
-            return sl["host"]
-        return [self.unpack(sl["host"][r], a["row"], a["T"]) for r in range(sl["host"].shape[0])]
+        host = sl["host"]
+        if self.grouping == "ae":
+            if float(host[:, :, -1].max()) > self.keep:
+                raise _lib.LitePoseError("an image holds more persons than the packed payload carries (%d): use step() "
+                                         "or a larger keep" % self.keep)
+            if not unpack:
+                return host
+        res = [self._decode(host[r]) for r in range(host.shape[0])]      # fast: raises on a KM status 1
+        return res if unpack else host
 
     def fetch_overflow(self, st, host):
         """Second-chance copy for the images that found more than ``keep`` persons: {image index: (ans, scores)} read
