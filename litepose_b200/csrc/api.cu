@@ -95,6 +95,28 @@ int make_tmap(CUtensorMap* map, const void* base, int rank, const uint64_t* dims
     return LP_OK;
 }
 
+int make_tmap_nhwc(CUtensorMap* map, const void* x, int N, int H, int W, int C, int box_c, int box_w, int box_h,
+                   CUtensorMapSwizzle swz) {
+    uint64_t dims[4] = {(uint64_t)C, (uint64_t)W, (uint64_t)H, (uint64_t)N};
+    uint64_t strides[3] = {(uint64_t)C * 2, (uint64_t)W * C * 2, (uint64_t)H * W * C * 2};
+    uint32_t box[4] = {(uint32_t)box_c, (uint32_t)box_w, (uint32_t)box_h, 1u};
+    return make_tmap(map, x, 4, dims, strides, box, swz);
+}
+
+int make_tmap_rows64(CUtensorMap* map, const void* w, int rows, int box_k, int box_rows, CUtensorMapSwizzle swz) {
+    uint64_t dims[2] = {64u, (uint64_t)rows};
+    uint64_t strides[1] = {128u};
+    uint32_t box[2] = {(uint32_t)box_k, (uint32_t)box_rows};
+    return make_tmap(map, w, 2, dims, strides, box, swz);
+}
+
+int make_tmap_taps(CUtensorMap* map, const void* w, int taps, int C) {
+    uint64_t dims[2] = {(uint64_t)C, (uint64_t)taps};
+    uint64_t strides[1] = {(uint64_t)C * 2};
+    uint32_t box[2] = {32u, (uint32_t)taps};
+    return make_tmap(map, w, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE);
+}
+
 int num_sms() {
     static thread_local int cached_dev = -1;
     static thread_local int cached = 0;

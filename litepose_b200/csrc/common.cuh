@@ -44,6 +44,14 @@ void count_launch();
 int make_tmap(CUtensorMap* map, const void* base, int rank, const uint64_t* dims,
               const uint64_t* strides_bytes, const uint32_t* box, CUtensorMapSwizzle swz,
               CUtensorMapDataType dt = CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
+// The fp16 layouts the kernels load:
+//   NHWC activation [N][H][W][C], box (box_c channels x box_w x box_h pixels) of one image
+int make_tmap_nhwc(CUtensorMap* map, const void* x, int N, int H, int W, int C, int box_c, int box_w, int box_h,
+                   CUtensorMapSwizzle swz);
+//   packed K-major weights [rows][64] (lp_pw1x1_pack and its kin), box (box_k columns x box_rows rows)
+int make_tmap_rows64(CUtensorMap* map, const void* w, int rows, int box_k, int box_rows, CUtensorMapSwizzle swz);
+//   tap-major depthwise weights [taps][C], box = every tap of one 32-channel slab, unswizzled
+int make_tmap_taps(CUtensorMap* map, const void* w, int taps, int C);
 
 int num_sms();
 
@@ -361,6 +369,33 @@ __device__ __forceinline__ void wg_mma_n(float (&acc)[NC][8], uint32_t a_addr, u
 // acc[c][2i], acc[c][2i+1] at row 16w + lane/4 + 8*(i&1), columns 16c + 8*(i>>1) + 2*(lane&3) + {0,1}.
 __device__ __forceinline__ int frag_row(int wq, int lane, int i) { return 16 * wq + (lane >> 2) + 8 * (i & 1); }
 __device__ __forceinline__ int frag_col(int lane, int i) { return 8 * (i >> 1) + 2 * (lane & 3); }
+
+// Projection epilogue of value pairs i of the NC chunks of an accumulator fragment (one pixel, NHWC element offset
+// off): out = fp16(acc + bias (+ residual)), the bias and residual added in fp32 and one rounding at the end.
+template <int NC>
+__device__ __forceinline__ void proj_store_row(__half* out, const __half* residual, size_t off, int Co,
+                                               const float (&acc)[NC][8], int i, const float* bias, int lane) {
+#pragma unroll
+    for (int c = 0; c < NC; ++c) {
+        const int co = c * 16 + frag_col(lane, i);
+        if (co >= Co) continue;
+        float2 v = make_float2(acc[c][2 * i] + bias[co], acc[c][2 * i + 1] + bias[co + 1]);
+        if (residual) {
+            const float2 f = __half22float2(*reinterpret_cast<const __half2*>(residual + off + co));
+            v.x += f.x;
+            v.y += f.y;
+        }
+        *reinterpret_cast<__half2*>(out + off + co) = __float22half2_rn(v);
+    }
+}
+
+__device__ __forceinline__ __half2 relu6_h2(__half2 v) {
+    return __hmin2(__hmax2(v, __floats2half2_rn(0.f, 0.f)), __floats2half2_rn(6.f, 6.f));
+}
+
+// Expansion epilogue: relu6(fp16(v)) for v = acc + bias in fp32.  The clamp runs on the rounded, packed pair and is
+// exact: rounding to fp16 is monotonic and 0 and 6 are fp16 values, so clamping commutes with it.
+__device__ __forceinline__ __half2 expand_relu6(float v0, float v1) { return relu6_h2(__floats2half2_rn(v0, v1)); }
 
 __device__ __forceinline__ float act_apply(float v, int act) {
     if (act == LP_ACT_RELU) return fmaxf(v, 0.f);

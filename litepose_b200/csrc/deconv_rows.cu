@@ -355,10 +355,7 @@ int launch_deconv_rows(const void* refined, const void* raw, const void* w_rows,
     p.pair_pitch = 4 * Co + 16;
     CUtensorMap mw;
     {
-        uint64_t dims[2] = {64, (uint64_t)16 * p.n_tile};
-        uint64_t strides[1] = {128};
-        uint32_t box[2] = {64, (uint32_t)p.n_tile};
-        int rc = make_tmap(&mw, w_rows, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
+        int rc = make_tmap_rows64(&mw, w_rows, 16 * p.n_tile, 64, p.n_tile, CU_TENSOR_MAP_SWIZZLE_128B);
         if (rc) return rc;
     }
     const size_t smem = dr_smem_bytes(Co);

@@ -9,7 +9,7 @@
 //     the tensor pipe is otherwise idle), fp32 accumulators in registers,
 //   * the same warps turn the accumulators (+bias -> ReLU6 -> zero outside the image -> fp16) into the [22][22][32ch]
 //     slab layout of the depthwise loop (the "epilogue" of the expansion),
-//   * run the packed-fp16 7x7 depthwise on the slab (same HFMA2 loop as dwpw.cu), write ReLU6'd fp16 results into
+//   * run the packed-fp16 7x7 depthwise on the slab (dw_inner.cuh, as in dwpw.cu), write ReLU6'd fp16 results into
 //     the swizzled K-major A tile; the four warpgroups then run the projection wgmma on 64 pixels each (fp32
 //     accumulators in registers for the whole tile),
 //   * all 16 depthwise warps finish the tile from their accumulators: + bias, + identity row (read back from
@@ -190,8 +190,8 @@ block_s1_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
         const int oy = by * 4, ox = bx * 4;
         uint8_t* slab = sSlab + grp * BK_SLAB;
         const uint32_t a_wg = smem_u32(sA + (wg >> 1) * BK_A_TILE) + (wg & 1) * 8192;
-        const __half2 zero2 = __floats2half2_rn(0.f, 0.f), six2 = __floats2half2_rn(6.f, 6.f);
-        uint32_t ec = 0;                                   // slabs expanded by this group
+        const __half2 zero2 = __floats2half2_rn(0.f, 0.f);
+        uint32_t ec = 0;                                  // slabs expanded by this group
         int it = 0;
         float pacc[NC][8];                                 // projection accumulators
         if (!STREAM) mbar_wait(&bars->w_full, 0);           // weights resident
@@ -258,8 +258,7 @@ block_s1_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
                             for (int k = 0; k < K16; ++k) wg_mma_n<2>(eacc[b], x_base + b * 8192 + k * 32, b_base + k * 32, k);
                         wg_commit();
                         wg_wait0();
-                        // + bias in fp32, round to fp16, ReLU6 on the packed halves (clamping commutes with rounding),
-                        // zero outside the image; chunk-major slab layout
+                        // expansion epilogue, zero outside the image; chunk-major slab layout
 #pragma unroll
                         for (int b = 0; b < 2; ++b)
 #pragma unroll
@@ -272,10 +271,8 @@ block_s1_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
                                     const int ch = c * 16 + frag_col(lane, i);
                                     __half2 h = zero2;
                                     if (in)
-                                        h = __hmin2(__hmax2(__floats2half2_rn(eacc[b][c][2 * i] + be[i >> 1][c][0],
-                                                                              eacc[b][c][2 * i + 1] + be[i >> 1][c][1]),
-                                                            zero2),
-                                                    six2);
+                                        h = expand_relu6(eacc[b][c][2 * i] + be[i >> 1][c][0],
+                                                         eacc[b][c][2 * i + 1] + be[i >> 1][c][1]);
                                     *reinterpret_cast<__half2*>(slab + (ch >> 3) * BK_CHUNK + pi * 16 + (ch & 7) * 2) = h;
                                 }
                             }
@@ -303,6 +300,7 @@ block_s1_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
                         dw_slab_hfma2<K, 4, BK_I, BK_CB, 4>(tile_in, reinterpret_cast<const __half2*>(sDww + s * BK_DW_SLAB), cp, mir,
                                                             oy, ox, bh, acch);
                     }
+                    dw_relu6(acch);
                 }
                 // the single A buffer is free once every warpgroup's projection MMAs of the previous K block retired
                 asm volatile("bar.sync 3, 512;" ::: "memory");
@@ -335,19 +333,7 @@ block_s1_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
                 const int py = (wg >> 1) * 8 + (row >> 4), px = row & 15;
                 const int gy = ty * BK_T + py, gx = tx * BK_T + px;
                 if (gy >= p.H || gx >= p.W) continue;
-                const size_t off = (((size_t)n * p.H + gy) * p.W + gx) * p.Co;
-#pragma unroll
-                for (int c = 0; c < NC; ++c) {
-                    const int co = c * 16 + frag_col(lane, i);
-                    if (co >= p.Co) continue;
-                    float2 v = make_float2(pacc[c][2 * i] + sBpj[co], pacc[c][2 * i + 1] + sBpj[co + 1]);
-                    if (p.residual) {
-                        const float2 f = __half22float2(*reinterpret_cast<const __half2*>(p.residual + off + co));
-                        v.x += f.x;
-                        v.y += f.y;
-                    }
-                    *reinterpret_cast<__half2*>(p.out + off + co) = __float22half2_rn(v);
-                }
+                proj_store_row<NC>(p.out, p.residual, (((size_t)n * p.H + gy) * p.W + gx) * p.Co, p.Co, pacc, i, sBpj, lane);
             }
         }
     }
@@ -410,10 +396,10 @@ __device__ __forceinline__ void s2_load_next_x(const CUtensorMap* map_x, S2Bars*
 }
 
 // expansion of slab s into `slab` for haloed pixels of M-tiles 2 mp0 .. 2 mp1 - 1 (one warpgroup, two M-tiles per
-// wgmma batch): + bias in fp32, round to fp16, ReLU6 (clamping commutes with rounding), zero outside the image
+// wgmma batch): the expansion epilogue, zero outside the image
 __device__ __forceinline__ void s2_expand(uint8_t* slab, const uint8_t* sX, const uint8_t* sWe, const float* sBexp, int s,
                                           int mp0, int mp1, uint32_t in_img, int wq, int lane) {
-    const __half2 zero2 = __floats2half2_rn(0.f, 0.f), six2 = __floats2half2_rn(6.f, 6.f);
+    const __half2 zero2 = __floats2half2_rn(0.f, 0.f);
     float be[2][2][2];
 #pragma unroll
     for (int i = 0; i < 2; ++i)
@@ -443,11 +429,7 @@ __device__ __forceinline__ void s2_expand(uint8_t* slab, const uint8_t* sX, cons
                 for (int c = 0; c < 2; ++c) {
                     const int ch = c * 16 + frag_col(lane, i);
                     __half2 h = zero2;
-                    if (in)
-                        h = __hmin2(__hmax2(__floats2half2_rn(eacc[b][c][2 * i] + be[i >> 1][c][0],
-                                                              eacc[b][c][2 * i + 1] + be[i >> 1][c][1]),
-                                            zero2),
-                                    six2);
+                    if (in) h = expand_relu6(eacc[b][c][2 * i] + be[i >> 1][c][0], eacc[b][c][2 * i + 1] + be[i >> 1][c][1]);
                     *reinterpret_cast<__half2*>(slab + pi * (S2_PP * 4) + ch * 2) = h;
                 }
             }
@@ -459,7 +441,6 @@ __device__ __forceinline__ void s2_expand(uint8_t* slab, const uint8_t* sX, cons
 template <int BY>
 __device__ __forceinline__ void s2_depthwise(const uint8_t* slab, const uint8_t* sDww, const float* sBdw, uint8_t* sA, int s,
                                              int cp, int oy, int ox) {
-    const __half2 zero2 = __floats2half2_rn(0.f, 0.f), six2 = __floats2half2_rn(6.f, 6.f);
     __half2 acch[BY][4];
     const __half2 bh = __float22half2_rn(*reinterpret_cast<const float2*>(sBdw + s * BK_CB + 2 * cp));
     dw_slab_hfma2<7, BY, S2_IW, BK_CB, S2_PP, 2>(reinterpret_cast<const __half2*>(slab) + cp,
@@ -471,8 +452,7 @@ __device__ __forceinline__ void s2_depthwise(const uint8_t* slab, const uint8_t*
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             const int r = (oy + i) * S2_TW + ox + j;
-            const __half2 v = __hmin2(__hmax2(acch[i][j], zero2), six2);
-            *reinterpret_cast<__half2*>(a_s + r * 64 + (((cp >> 2) ^ ((r >> 1) & 3)) << 4) + ((cp & 3) << 2)) = v;
+            *reinterpret_cast<__half2*>(a_s + r * 64 + (((cp >> 2) ^ ((r >> 1) & 3)) << 4) + ((cp & 3) << 2)) = relu6_h2(acch[i][j]);
         }
 }
 
@@ -601,14 +581,7 @@ block_s2_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
             const int row = wg * 64 + frag_row(wq, lane, i);
             const int gy = ty * S2_TH + (row >> 4), gx = tx * S2_TW + (row & 15);
             if (gy >= p.Hout || gx >= p.Wout) continue;
-            const size_t off = (((size_t)n * p.Hout + gy) * p.Wout + gx) * p.Co;
-#pragma unroll
-            for (int c = 0; c < NC; ++c) {
-                const int co = c * 16 + frag_col(lane, i);
-                if (co >= p.Co) continue;
-                *reinterpret_cast<__half2*>(p.out + off + co) =
-                    __float22half2_rn(make_float2(pacc[c][2 * i] + sBpj[co], pacc[c][2 * i + 1] + sBpj[co + 1]));
-            }
+            proj_store_row<NC>(p.out, nullptr, (((size_t)n * p.Hout + gy) * p.Wout + gx) * p.Co, p.Co, pacc, i, sBpj, lane);
         }
     }
 }
@@ -703,28 +676,14 @@ extern "C" int lp_block_s1_f16(const void* x, const void* w_exp_packed, const fl
     p.residual = identity ? reinterpret_cast<const __half*>(x) : nullptr;
     p.out = reinterpret_cast<__half*>(out);
     CUtensorMap mx, mwe, mdw, mwp;
-    {
-        uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)N};
-        uint64_t strides[3] = {(uint64_t)Cin * 2, (uint64_t)W * Cin * 2, (uint64_t)H * W * Cin * 2};
-        uint32_t box[4] = {64u, (uint32_t)BK_I, (uint32_t)BK_I, 1u};
-        int rc = make_tmap(&mx, x, 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
-        if (rc) return rc;
-        uint64_t d2[2] = {64u, (uint64_t)p.nslabs * BK_CB};
-        uint64_t s2[1] = {128u};
-        uint32_t b2[2] = {64u, (uint32_t)BK_CB};
-        rc = make_tmap(&mwe, w_exp_packed, 2, d2, s2, b2, CU_TENSOR_MAP_SWIZZLE_128B);
-        if (rc) return rc;
-        uint64_t d3[2] = {(uint64_t)Ce, 49u};
-        uint64_t s3[1] = {(uint64_t)Ce * 2};
-        uint32_t b3[2] = {(uint32_t)BK_CB, 49u};
-        rc = make_tmap(&mdw, w_dw, 2, d3, s3, b3, CU_TENSOR_MAP_SWIZZLE_NONE);
-        if (rc) return rc;
-        uint64_t d4[2] = {64u, (uint64_t)p.nkb * p.n_tile};
-        uint64_t s4[1] = {128u};
-        uint32_t b4[2] = {64u, (uint32_t)p.n_tile};
-        rc = make_tmap(&mwp, w_proj_packed, 2, d4, s4, b4, CU_TENSOR_MAP_SWIZZLE_128B);
-        if (rc) return rc;
-    }
+    int rc = make_tmap_nhwc(&mx, x, N, H, W, Cin, 64, BK_I, BK_I, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (rc) return rc;
+    rc = make_tmap_rows64(&mwe, w_exp_packed, p.nslabs * BK_CB, 64, BK_CB, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (rc) return rc;
+    rc = make_tmap_taps(&mdw, w_dw, 49, Ce);
+    if (rc) return rc;
+    rc = make_tmap_rows64(&mwp, w_proj_packed, p.nkb * p.n_tile, 64, p.n_tile, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (rc) return rc;
     const int grid = p.num_tiles < num_sms() ? p.num_tiles : num_sms();
     const int nc = p.n_tile / 16;
     using Kern = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const BkParams);
@@ -790,29 +749,15 @@ extern "C" int lp_block_s2_f16(const void* x, const void* w_exp_packed, const fl
     p.b_pj = b_proj_packed;
     p.out = reinterpret_cast<__half*>(out);
     CUtensorMap mx, mwe, mdw, mwp;
-    {
-        uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)N};
-        uint64_t strides[3] = {(uint64_t)Cin * 2, (uint64_t)W * Cin * 2, (uint64_t)H * W * Cin * 2};
-        uint32_t box[4] = {16u, (uint32_t)S2_IW, (uint32_t)S2_IH, 1u};
-        int rc = make_tmap(&mx, x, 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_32B);
-        if (rc) return rc;
-        // the K = 16 slice (columns 0..15) of lp_block_s1_pack_wexp's [nslabs*32][64] rows
-        uint64_t d2[2] = {64u, (uint64_t)p.nslabs * BK_CB};
-        uint64_t s2[1] = {128u};
-        uint32_t b2[2] = {16u, (uint32_t)BK_CB};
-        rc = make_tmap(&mwe, w_exp_packed, 2, d2, s2, b2, CU_TENSOR_MAP_SWIZZLE_32B);
-        if (rc) return rc;
-        uint64_t d3[2] = {(uint64_t)Ce, 49u};
-        uint64_t s3[1] = {(uint64_t)Ce * 2};
-        uint32_t b3[2] = {(uint32_t)BK_CB, 49u};
-        rc = make_tmap(&mdw, w_dw, 2, d3, s3, b3, CU_TENSOR_MAP_SWIZZLE_NONE);
-        if (rc) return rc;
-        uint64_t d4[2] = {64u, (uint64_t)p.nkb * p.n_tile};
-        uint64_t s4[1] = {128u};
-        uint32_t b4[2] = {64u, (uint32_t)p.n_tile};
-        rc = make_tmap(&mwp, w_proj_packed, 2, d4, s4, b4, CU_TENSOR_MAP_SWIZZLE_128B);
-        if (rc) return rc;
-    }
+    int rc = make_tmap_nhwc(&mx, x, N, H, W, Cin, 16, S2_IW, S2_IH, CU_TENSOR_MAP_SWIZZLE_32B);
+    if (rc) return rc;
+    // the K = 16 slice (columns 0..15) of lp_block_s1_pack_wexp's [nslabs*32][64] rows
+    rc = make_tmap_rows64(&mwe, w_exp_packed, p.nslabs * BK_CB, 16, BK_CB, CU_TENSOR_MAP_SWIZZLE_32B);
+    if (rc) return rc;
+    rc = make_tmap_taps(&mdw, w_dw, 49, Ce);
+    if (rc) return rc;
+    rc = make_tmap_rows64(&mwp, w_proj_packed, p.nkb * p.n_tile, 64, p.n_tile, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (rc) return rc;
     const int grid = p.num_tiles < num_sms() ? p.num_tiles : num_sms();
     using Kern = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const S2Params);
     static const Kern kernels[4] = {block_s2_kernel<1>, block_s2_kernel<2>, block_s2_kernel<3>, block_s2_kernel<4>};

@@ -7,9 +7,11 @@
 // input tile is staged in shared memory by ONE TMA tensor copy (cp.async.bulk.tensor.4d) whose
 // out-of-bounds zero fill implements the conv padding and every image/channel border, so the
 // compute loop has no boundary branches.  Each thread owns one channel PAIR (half2) and walks
-// 4x4 output micro-blocks with the k*k half2 weights held in registers, accumulating in fp32.
+// 4x4 output micro-blocks with the k*k half2 weights held in registers; the arithmetic of each precision mode is
+// dw_inner.cuh's (packed fp16 chains, fp32 FMA per product, or packed row sums added in fp32).
 // Algorithmic bytes per launch: 2*(N*C*Hin*Win + N*C*Hout*Wout + C*k*k) (+4*C bias).
 #include "common.cuh"
+#include "dw_inner.cuh"
 
 namespace lp {
 
@@ -23,22 +25,10 @@ struct DwCfg {
     static constexpr int TW = (S == 1) ? 32 : 16;
     static constexpr int IH = (TH - 1) * S + K;             // input tile incl. halo
     static constexpr int IW = (TW - 1) * S + K;
-    static constexpr int IR = (BY - 1) * S + K;             // input rows / cols per micro-block
-    static constexpr int IC = (BX - 1) * S + K;
     static constexpr int SMEM = IH * IW * DW_CB * 2 + 128 + 64;
 };
 
-// fp16 x fp16 + fp32 -> fp32 with one rounding: the fp16 -> fp32 conversions are exact, so the fp32 FMA of the
-// converted operands gives the same result as a mixed-precision FMA.
-__device__ __forceinline__ float fhfma(unsigned short a, unsigned short b, float c) {
-    return __fmaf_rn(__half2float(__ushort_as_half(a)), __half2float(__ushort_as_half(b)), c);
-}
-__device__ __forceinline__ float fhadd(unsigned short a, float c) { return __fadd_rn(__half2float(__ushort_as_half(a)), c); }
-__device__ __forceinline__ unsigned short lo16(__half2 v) { return __half_as_ushort(__low2half(v)); }
-__device__ __forceinline__ unsigned short hi16(__half2 v) { return __half_as_ushort(__high2half(v)); }
-
-// PREC 0: every product accumulated in fp32 (fhfma).  PREC 1: the K taps of one kernel row are accumulated with
-// packed HFMA2 in fp16 (2 channels per instruction), each row sum is then added into the fp32 accumulator (fhadd).
+// PREC: the precision mode of dw_inner.cuh (0 dw_ffma, 1 dw_rowsum, 2 dw_hfma2).
 template <int K, int S, int PREC>
 __global__ void __launch_bounds__(DW_THREADS, 2)
 dwconv_kernel(const __grid_constant__ CUtensorMap map_x, const __half* __restrict__ w, const float* __restrict__ bias,
@@ -86,10 +76,9 @@ dwconv_kernel(const __grid_constant__ CUtensorMap map_x, const __half* __restric
     pdl_wait();               // also orders this kernel's output writes after the previous kernel's reads
     mbar_wait(bar, 0);
 
-    const __half2* tile_in = reinterpret_cast<const __half2*>(smem);   // [IH][IW][16 pairs]
+    const __half2* tile_in = reinterpret_cast<const __half2*>(smem) + cp;   // [IH][IW][16 pairs], this thread's pair
     constexpr int PAIRS_X = Cfg::TW / (2 * BX);
     constexpr int NPAIRS = (Cfg::TH / BY) * PAIRS_X;
-    const int cstep = mir ? -(DW_CB / 2) : (DW_CB / 2);
 
 #pragma unroll 1
     for (int q = wid; q < NPAIRS; q += DW_THREADS / 32) {
@@ -97,65 +86,10 @@ dwconv_kernel(const __grid_constant__ CUtensorMap map_x, const __half* __restric
         const int oy = by * BY, ox = bx * BX;           // tile-local output origin
         if (oy0 + oy >= Hout || ox0 + ox >= Wout) continue;   // micro-block fully outside
         float2 acc[BY][BX];
-        __half2 acch[BY][BX], part[BY][BX];      // PREC 2: running fp16 total + current two-row chain
-        const __half2 bh = __float22half2_rn(b2);
-#pragma unroll
-        for (int i = 0; i < BY; ++i)
-#pragma unroll
-            for (int j = 0; j < BX; ++j) {
-                acc[i][j] = b2;
-                acch[i][j] = bh;
-            }
-
-        // slot c of a row holds input column (ox*S + c), or (ox*S + IC-1-c) when mirrored
-        const __half2* base = tile_in + ((oy * S) * Cfg::IW + ox * S + (mir ? Cfg::IC - 1 : 0)) * (DW_CB / 2) + cp;
-#pragma unroll
-        for (int r = 0; r < Cfg::IR; ++r) {
-            __half2 in[Cfg::IC];
-#pragma unroll
-            for (int c = 0; c < Cfg::IC; ++c) in[c] = base[r * Cfg::IW * (DW_CB / 2) + c * cstep];
-#pragma unroll
-            for (int i = 0; i < BY; ++i) {
-                const int ky = r - i * S;
-                if (ky >= 0 && ky < K) {
-                    if (PREC == 0) {
-#pragma unroll
-                        for (int kx = 0; kx < K; ++kx) {
-                            const __half2 wv = wreg[ky * K + kx];
-#pragma unroll
-                            for (int j = 0; j < BX; ++j) {
-                                acc[i][j].x = fhfma(lo16(in[j * S + kx]), lo16(wv), acc[i][j].x);
-                                acc[i][j].y = fhfma(hi16(in[j * S + kx]), hi16(wv), acc[i][j].y);
-                            }
-                        }
-                    } else if (PREC == 2) {
-                        // fully packed: chains of two kernel rows folded into a running fp16 total (dw_inner.cuh)
-#pragma unroll
-                        for (int kx = 0; kx < K; ++kx) {
-                            const __half2 wv = wreg[ky * K + kx];
-#pragma unroll
-                            for (int j = 0; j < BX; ++j) {
-                                if ((ky & 1) == 0 && kx == 0) part[i][j] = __hmul2(in[j * S + kx], wv);
-                                else part[i][j] = __hfma2(in[j * S + kx], wv, part[i][j]);
-                            }
-                        }
-                        if ((ky & 1) || ky == K - 1) {
-#pragma unroll
-                            for (int j = 0; j < BX; ++j) acch[i][j] = __hadd2(acch[i][j], part[i][j]);
-                        }
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < BX; ++j) {
-                            __half2 sacc = __hmul2(in[j * S], wreg[ky * K]);
-#pragma unroll
-                            for (int kx = 1; kx < K; ++kx) sacc = __hfma2(in[j * S + kx], wreg[ky * K + kx], sacc);
-                            acc[i][j].x = fhadd(lo16(sacc), acc[i][j].x);
-                            acc[i][j].y = fhadd(hi16(sacc), acc[i][j].y);
-                        }
-                    }
-                }
-            }
-        }
+        __half2 acch[BY][BX];
+        if constexpr (PREC == 0) dw_ffma<K, BY, Cfg::IW, DW_CB / 2, S>(tile_in, wreg, mir, oy, ox, b2, acc);
+        else if constexpr (PREC == 1) dw_rowsum<K, BY, Cfg::IW, DW_CB / 2, S>(tile_in, wreg, mir, oy, ox, b2, acc);
+        else dw_hfma2<K, BY, Cfg::IW, DW_CB / 2, S>(tile_in, wreg, mir, oy, ox, __float22half2_rn(b2), acch);
         if (ch_ok) {
             const int gy0 = oy0 + oy, gx0 = ox0 + ox;
             // one 64-bit base per micro-block; every pixel is base + (i*Wout + jj)*C elements
@@ -198,10 +132,7 @@ static int launch_dw(const void* x, const void* w, const float* bias, void* y, i
     using Cfg = DwCfg<K, S>;
     const int Hout = H / S, Wout = W / S;
     CUtensorMap map;
-    uint64_t dims[4] = {(uint64_t)C, (uint64_t)W, (uint64_t)H, (uint64_t)N};
-    uint64_t strides[3] = {(uint64_t)C * 2, (uint64_t)W * C * 2, (uint64_t)H * W * C * 2};
-    uint32_t box[4] = {(uint32_t)DW_CB, (uint32_t)Cfg::IW, (uint32_t)Cfg::IH, 1u};
-    int rc = make_tmap(&map, x, 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE);
+    int rc = make_tmap_nhwc(&map, x, N, H, W, C, DW_CB, Cfg::IW, Cfg::IH, CU_TENSOR_MAP_SWIZZLE_NONE);
     if (rc) return rc;
     cudaError_t e = cudaFuncSetAttribute((const void*)dwconv_kernel<K, S, PREC>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);

@@ -7,13 +7,14 @@
 //   warp 16 (1 thread) TMA producer: haloed 22x22x32-channel input slabs (hardware zero fill = conv padding) into a
 //                      4-deep ring, projection-weight K blocks into a 2-deep ring
 //   warps 0-15         depthwise on the CUDA cores, two groups of 8 warps working on the two 32-channel halves of a
-//                      64-channel K block: one 4x4 micro-block x channel pair per thread per slab; blocks (HEAD = 0):
-//                      packed fp16 HFMA2 in chains of two kernel rows folded into a running fp16 total, heads
-//                      (HEAD = 1): fp32 accumulation; mirrored conflict-free LDS as in dwconv.cu; results written as
-//                      fp16 straight into the 128B-swizzled K-major A-operand tiles
+//                      64-channel K block: one 4x4 micro-block x channel pair per thread per slab, with the arithmetic
+//                      of dw_inner.cuh: blocks (HEAD = 0) its packed-fp16 chains (dw_slab_hfma2), heads (HEAD = 1) its
+//                      fp32 accumulation (dw_ffma); results written as fp16 straight into the 128B-swizzled K-major
+//                      A-operand tiles (dw_store_a)
 //   warps 0-15         as four warpgroups, one per 64 pixels: wgmma D[64 px x Co] += A[64 x 64 ch] * Wp^T per
 //                      64-channel K block, fp32 accumulators in registers; then the epilogue from the accumulator
-//                      fragments: + folded-BN bias (+ residual), fp16 NHWC (heads: NCHW fp32/fp16 planes)
+//                      fragments: + folded-BN bias (+ residual), fp16 NHWC (proj_store_row; heads: NCHW fp32/fp16
+//                      planes)
 // HBM traffic per block: read N*H*W*Ce*2 (+ N*H*W*Co*2 residual), write N*H*W*Co*2  -- the depthwise output
 // (N*H*W*Ce*2 written + read again) is gone; the kernel is bound by the FMA pipe (2*49 flop per expanded element).
 #include "common.cuh"
@@ -27,7 +28,6 @@ template <int K> struct FpCfg {
     static constexpr int I = FP_T + K - 1;                       // haloed input side (22 for k = 7, 20 for k = 5)
     static constexpr int IN_BYTES = I * I * FP_CB * 2;           // 30976 / 25600
     static constexpr int W_BYTES = K * K * FP_CB * 2;            // depthwise weights of one slab: 3136 / 1600 B
-    static constexpr int IR = 4 + K - 1;                         // input rows / columns of a 4x4 micro-block
 };
 constexpr int FP_IN_STRIDE = 35840;                           // ring pitch: input tile + weight slab (multiple of 1024)
 constexpr int FP_W_OFF = 31744;                               // weights inside a ring stage (128-byte aligned)
@@ -63,13 +63,6 @@ struct FpParams {
     const __half* residual;           // [N,H,W,Co] or null
     void* out;                        // [N,H,W,Co] fp16 (HEAD: [N,Co,H,W] fp32/fp16)
 };
-
-// fp16 x fp16 + fp32 -> fp32, one rounding (the fp16 -> fp32 conversions are exact)
-__device__ __forceinline__ float fp_fhfma(unsigned short a, unsigned short b, float c) {
-    return __fmaf_rn(__half2float(__ushort_as_half(a)), __half2float(__ushort_as_half(b)), c);
-}
-__device__ __forceinline__ unsigned short fp_lo(__half2 v) { return __half_as_ushort(__low2half(v)); }
-__device__ __forceinline__ unsigned short fp_hi(__half2 v) { return __half_as_ushort(__high2half(v)); }
 
 // HEAD = 0: block projection (ReLU6 after the depthwise, NHWC fp16 output with bias and optional residual).
 // HEAD = 1: output head (two sources, ReLU after the depthwise, bias-free 1x1, NCHW fp32/fp16 output).
@@ -146,8 +139,7 @@ dw_project_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_consta
         const int blk = (gw << 1) | sub;                   // 16 micro-blocks: 4 x 4 of 4x4 pixels
         const int by = blk >> 2, bx = blk & 3;
         const int oy = by * 4, ox = bx * 4;
-        const int cstep = mir ? -(FP_CB / 2) : (FP_CB / 2);
-        uint32_t iu = 0;                                   // slabs consumed by this group
+        uint32_t iu = 0;                                  // slabs consumed by this group
         // ---- MMA warpgroup wg = warp / 4 owns pixels 64*wg .. 64*wg+63 of the 256-pixel tile (M-tile wg / 2)
         const int wg = warp >> 2, wq = warp & 3;
         const int nch = p.n_tile >> 4;
@@ -162,13 +154,12 @@ dw_project_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_consta
                 const int py = (wg >> 1) * 8 + (row >> 4), px = row & 15;
                 const int gy = ty * FP_T + py, gx = tx * FP_T + px;
                 if (gy >= p.H || gx >= p.W) continue;
-                const size_t off = (((size_t)n * p.H + gy) * p.W + gx) * p.Co;
+                if constexpr (HEAD) {
 #pragma unroll
-                for (int c = 0; c < NC; ++c) {
-                    const int co = c * 16 + frag_col(lane, i);
-                    if (c >= nch || co >= p.Co) continue;
-                    const float v0 = pacc[c][2 * i], v1 = pacc[c][2 * i + 1];
-                    if (HEAD) {
+                    for (int c = 0; c < NC; ++c) {
+                        const int co = c * 16 + frag_col(lane, i);
+                        if (co >= p.Co) continue;
+                        const float v0 = pacc[c][2 * i], v1 = pacc[c][2 * i + 1];
                         const size_t plane = (size_t)p.H * p.W;
                         const size_t o = ((size_t)n * p.Co + co) * plane + (size_t)gy * p.W + gx;
                         if (p.out_fp32) {
@@ -180,15 +171,10 @@ dw_project_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_consta
                             op[0] = __float2half_rn(v0);
                             if (co + 1 < p.Co) op[plane] = __float2half_rn(v1);
                         }
-                    } else {
-                        float2 v = make_float2(v0 + sBias[co], v1 + sBias[co + 1]);
-                        if (p.residual) {
-                            const float2 f = __half22float2(*reinterpret_cast<const __half2*>(p.residual + off + co));
-                            v.x += f.x;
-                            v.y += f.y;
-                        }
-                        *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(p.out) + off + co) = __float22half2_rn(v);
                     }
+                } else {
+                    proj_store_row<NC>(reinterpret_cast<__half*>(p.out), p.residual, (((size_t)n * p.H + gy) * p.W + gx) * p.Co,
+                                       p.Co, pacc, i, sBias, lane);
                 }
             }
         };
@@ -204,74 +190,23 @@ dw_project_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_consta
                 // smaller micro-blocks need more LDS per MAC.)
                 const int s = 2 * kb + grp;
                 const bool have = s < p.nslabs;            // the last K block may hold a single slab
-                // Accumulators.  Blocks (HEAD = 0): packed fp16 (HFMA2, two channels per instruction, 2 MACs per lane
-                // per instruction, where the fp32 chain below needs an issue slot per MAC-lane).  The 49 taps are accumulated as four fp16 chains (two kernel rows each) folded into a
-                // running fp16 total: the network stays at 0.27-0.34 of the parity tolerance for XS/S, 0.67 for M 512
-                // (0.25-0.30 and 0.62 with an fp32 depthwise; the error budget is dominated by the fp16 activation
-                // storage; bit-exact emulation in tests/emulate_dw_precision.py).  Heads (HEAD = 1) feed the network
-                // outputs directly and keep fp32 accumulation.
+                // Depthwise (dw_inner.cuh): blocks (HEAD = 0) run the packed-fp16 chains; the heads (HEAD = 1) feed the
+                // network outputs directly and keep fp32 accumulation.  The slab's weights are TMA-staged next to its
+                // input tile ([K*K][32] fp16; channels beyond Ce are zero-filled by the tensor map).
                 float2 acc[4][4];
-                __half2 acch[4][4], part[4][4];
+                __half2 acch[4][4];
                 if (have) {
-                    const int ch = s * FP_CB + 2 * cp;
-                    const float2 b2 = *reinterpret_cast<const float2*>(sBdw + ch);
-                    const __half2 bh = __float22half2_rn(b2);
-#pragma unroll
-                    for (int i = 0; i < 4; ++i)
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            acc[i][j] = b2;
-                            acch[i][j] = bh;
-                        }
-
+                    const float2 b2 = *reinterpret_cast<const float2*>(sBdw + s * FP_CB + 2 * cp);
                     const uint32_t is = 2 * (iu & 1) + grp;          // this group's stages: grp, grp+2
                     mbar_wait(&bars->in_full[is], (iu >> 1) & 1);
-                    // weights of this slab (TMA-staged next to the input tile, [49][32] fp16; channels beyond Ce are
-                    // zero-filled by the tensor map); mirrored lanes read kx reversed
-                    __half2 wreg[K * K];
-                    {
-                        const __half2* ws = reinterpret_cast<const __half2*>(sIn + is * FP_IN_STRIDE + FP_W_OFF) + cp +
-                                            (mir ? (K - 1) * (FP_CB / 2) : 0);
-                        const int wstep = mir ? -(FP_CB / 2) : (FP_CB / 2);
-#pragma unroll
-                        for (int ky = 0; ky < K; ++ky)
-#pragma unroll
-                            for (int kx = 0; kx < K; ++kx) wreg[ky * K + kx] = ws[ky * K * (FP_CB / 2) + kx * wstep];
-                    }
-                    const __half2* tile_in = reinterpret_cast<const __half2*>(sIn + is * FP_IN_STRIDE);
-                    const __half2* base = tile_in + (oy * FP_I + ox + (mir ? Cfg::IR - 1 : 0)) * (FP_CB / 2) + cp;
-#pragma unroll
-                    for (int r = 0; r < Cfg::IR; ++r) {
-                        __half2 in[Cfg::IR];
-#pragma unroll
-                        for (int c = 0; c < Cfg::IR; ++c) in[c] = base[r * FP_I * (FP_CB / 2) + c * cstep];
-#pragma unroll
-                        for (int i = 0; i < 4; ++i) {
-                            const int ky = r - i;
-                            if (ky >= 0 && ky < K) {
-#pragma unroll
-                                for (int kx = 0; kx < K; ++kx) {
-                                    const __half2 wv = wreg[ky * K + kx];
-#pragma unroll
-                                    for (int j = 0; j < 4; ++j) {
-                                        if (HEAD) {
-                                            acc[i][j].x = fp_fhfma(fp_lo(in[j + kx]), fp_lo(wv), acc[i][j].x);
-                                            acc[i][j].y = fp_fhfma(fp_hi(in[j + kx]), fp_hi(wv), acc[i][j].y);
-                                        } else if ((ky & 1) == 0 && kx == 0) {
-                                            part[i][j] = __hmul2(in[j + kx], wv);       // a new group of two kernel rows
-                                        } else {
-                                            part[i][j] = __hfma2(in[j + kx], wv, part[i][j]);
-                                        }
-                                    }
-                                }
-                                // fold the finished group (kernel rows {0,1},{2,3},{4,5},{6}) into the running total:
-                                // chains of <= 14 roundings at partial magnitude instead of 49 at full magnitude
-                                if (!HEAD && ((ky & 1) || ky == K - 1)) {
-#pragma unroll
-                                    for (int j = 0; j < 4; ++j) acch[i][j] = __hadd2(acch[i][j], part[i][j]);
-                                }
-                            }
-                        }
+                    const __half2* tile_in = reinterpret_cast<const __half2*>(sIn + is * FP_IN_STRIDE) + cp;
+                    const __half2* wslab = reinterpret_cast<const __half2*>(sIn + is * FP_IN_STRIDE + FP_W_OFF);
+                    if constexpr (HEAD) {
+                        __half2 wreg[K * K];
+                        dw_load_wslab<K, FP_CB>(wslab, cp, mir, wreg);
+                        dw_ffma<K, 4, FP_I, FP_CB / 2>(tile_in, wreg, mir, oy, ox, b2, acc);
+                    } else {
+                        dw_slab_hfma2<K, 4, FP_I, FP_CB>(tile_in, wslab, cp, mir, oy, ox, __float22half2_rn(b2), acch);
                     }
                     __syncwarp();
                     if (lane == 0) mbar_arrive(&bars->in_empty[is]);
@@ -280,22 +215,17 @@ dw_project_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_consta
                 // the single A buffer is free once every warpgroup's MMAs of the previous K block have retired
                 fp_dw_sync();
                 if (have) {
-                    // ReLU6, fp16, into the swizzled A tile: row = pixel, 16-byte chunk j = channels 8j..8j+7 of the K block
-                    uint8_t* a_mt = sA + (by >> 1) * FP_A_TILE;
-                    const int jch = (grp << 2) | (cp >> 2);
-                    const __half2 zero2 = __floats2half2_rn(0.f, 0.f), six2 = __floats2half2_rn(6.f, 6.f);
+                    if constexpr (HEAD) {
+                        // ReLU in fp32, then one rounding (a packed hmax after rounding could turn +0 into -0)
 #pragma unroll
-                    for (int i = 0; i < 4; ++i)
+                        for (int i = 0; i < 4; ++i)
 #pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            const int r = ((oy + i) & 7) * 16 + ox + (mir ? 3 - j : j);     // row inside the M-tile
-                            __half2 v;
-                            if (HEAD)       // ReLU (heads)
-                                v = __floats2half2_rn(fmaxf(acc[i][j].x, 0.f), fmaxf(acc[i][j].y, 0.f));
-                            else            // ReLU6 (blocks), packed
-                                v = __hmin2(__hmax2(acch[i][j], zero2), six2);
-                            *reinterpret_cast<__half2*>(a_mt + r * 128 + ((jch ^ (r & 7)) << 4) + ((cp & 3) << 2)) = v;
-                        }
+                            for (int j = 0; j < 4; ++j)
+                                acch[i][j] = __floats2half2_rn(fmaxf(acc[i][j].x, 0.f), fmaxf(acc[i][j].y, 0.f));
+                    } else {
+                        dw_relu6(acch);
+                    }
+                    dw_store_a<4>(sA, FP_A_TILE, acch, oy, ox, mir, (grp << 2) | (cp >> 2), cp);
                     fence_proxy_async();
                 }
                 fp_dw_sync();                              // A tile complete
@@ -453,7 +383,7 @@ dw_project_wide_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_c
                     const __half2 bh = __float22half2_rn(*reinterpret_cast<const float2*>(sBdw + s * FP_CB + 2 * cp));
                     mbar_wait(&bars->in_full[is], (iu >> 1) & 1);
                     const uint8_t* st = sIn + is * FW_IN_STRIDE;
-                    dw_slab_hfma2<7, 4, FW_IX, FP_CB>(reinterpret_cast<const __half2*>(st),
+                    dw_slab_hfma2<7, 4, FW_IX, FP_CB>(reinterpret_cast<const __half2*>(st) + cp,
                                                       reinterpret_cast<const __half2*>(st + FW_W_OFF), cp, mir, oy, ox, bh, acch);
                     __syncwarp();
                     if (lane == 0) mbar_arrive(&bars->in_empty[is]);
@@ -462,6 +392,7 @@ dw_project_wide_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_c
                 const uint32_t q = au & 1;
                 mbar_wait(&bars->a_empty[q], ((au >> 1) & 1) ^ 1);
                 if (have) {
+                    dw_relu6(acch);
                     dw_store_a<4>(sA + q * FP_A_TILE, FP_A_TILE, acch, oy, ox, mir, jch, cp);
                     fence_proxy_async();
                 }
@@ -518,19 +449,8 @@ dw_project_wide_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_c
                 const int row = wg * 64 + frag_row(wq, lane, i);
                 const int gy = ty * FW_TY + (row >> 4), gx = tx * FW_TX + (row & 15);
                 if (gy >= p.H || gx >= p.W) continue;
-                const size_t off = (((size_t)n * p.H + gy) * p.W + gx) * p.Co;
-#pragma unroll
-                for (int c = 0; c < NC; ++c) {
-                    const int co = c * 16 + frag_col(lane, i);
-                    if (co >= p.Co) continue;
-                    float2 v = make_float2(pacc[c][2 * i] + sBias[co], pacc[c][2 * i + 1] + sBias[co + 1]);
-                    if (p.residual) {
-                        const float2 f = __half22float2(*reinterpret_cast<const __half2*>(p.residual + off + co));
-                        v.x += f.x;
-                        v.y += f.y;
-                    }
-                    *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(p.out) + off + co) = __float22half2_rn(v);
-                }
+                proj_store_row<NC>(reinterpret_cast<__half*>(p.out), p.residual, (((size_t)n * p.H + gy) * p.W + gx) * p.Co, p.Co,
+                                   pacc, i, sBias, lane);
             }
         }
     }
@@ -597,28 +517,15 @@ extern "C" int lp_dw7_project_f16(const void* x, const void* w_dw, const float* 
     p.residual = reinterpret_cast<const __half*>(residual);
     p.out = out;
     p.ns0 = p.nslabs;
-    CUtensorMap mx, mw;
-    {
-        uint64_t dims[4] = {(uint64_t)Ce, (uint64_t)W, (uint64_t)H, (uint64_t)N};
-        uint64_t strides[3] = {(uint64_t)Ce * 2, (uint64_t)W * Ce * 2, (uint64_t)H * W * Ce * 2};
-        uint32_t box[4] = {(uint32_t)FP_CB, (uint32_t)(wide ? FW_IX : FpCfg<7>::I), (uint32_t)(wide ? FW_IY : FpCfg<7>::I), 1u};
-        int rc = make_tmap(&mx, x, 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE);
-        if (rc) return rc;
-        // packed projection weights: [kb][n_tile][64] (lp_pw1x1_pack with a single N chunk since Co <= 160)
-        uint64_t d2[2] = {64u, (uint64_t)p.nkb * p.n_tile};
-        uint64_t s2[1] = {128u};
-        uint32_t b2[2] = {64u, (uint32_t)p.n_tile};
-        rc = make_tmap(&mw, w_proj_packed, 2, d2, s2, b2, CU_TENSOR_MAP_SWIZZLE_128B);
-        if (rc) return rc;
-    }
-    CUtensorMap md;
-    {
-        uint64_t d2[2] = {(uint64_t)Ce, 49u};
-        uint64_t s2[1] = {(uint64_t)Ce * 2};
-        uint32_t b2[2] = {(uint32_t)FP_CB, 49u};
-        int rc = make_tmap(&md, w_dw, 2, d2, s2, b2, CU_TENSOR_MAP_SWIZZLE_NONE);
-        if (rc) return rc;
-    }
+    CUtensorMap mx, mw, md;
+    int rc = make_tmap_nhwc(&mx, x, N, H, W, Ce, FP_CB, wide ? FW_IX : FpCfg<7>::I, wide ? FW_IY : FpCfg<7>::I,
+                            CU_TENSOR_MAP_SWIZZLE_NONE);
+    if (rc) return rc;
+    // packed projection weights: [kb][n_tile][64] (lp_pw1x1_pack with a single N chunk since Co <= 160)
+    rc = make_tmap_rows64(&mw, w_proj_packed, p.nkb * p.n_tile, 64, p.n_tile, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (rc) return rc;
+    rc = make_tmap_taps(&md, w_dw, 49, Ce);
+    if (rc) return rc;
     if (wide) return launch_dw_project_wide(mx, mw, md, p, (cudaStream_t)stream);
     return launch_dw_project<7, 0>(mx, mx, mw, md, p, (cudaStream_t)stream);
 }
@@ -698,25 +605,13 @@ extern "C" int lp_head_fused_f16(const void* a1, const void* a2, const void* dw_
     p.out = out_nchw;
     p.out_fp32 = out_fp32;
     CUtensorMap m0, m1, mw, md;
-    for (int i = 0; i < 2; ++i) {
-        const int C = i ? C2 : C1;
-        uint64_t dims[4] = {(uint64_t)C, (uint64_t)W, (uint64_t)H, (uint64_t)N};
-        uint64_t strides[3] = {(uint64_t)C * 2, (uint64_t)W * C * 2, (uint64_t)H * W * C * 2};
-        uint32_t box[4] = {(uint32_t)FP_CB, (uint32_t)FpCfg<5>::I, (uint32_t)FpCfg<5>::I, 1u};
-        int rc = make_tmap(i ? &m1 : &m0, i ? a2 : a1, 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE);
-        if (rc) return rc;
-    }
-    {
-        uint64_t d2[2] = {64u, (uint64_t)p.nkb * p.n_tile};
-        uint64_t s2[1] = {128u};
-        uint32_t b2[2] = {64u, (uint32_t)p.n_tile};
-        int rc = make_tmap(&mw, pw_packed, 2, d2, s2, b2, CU_TENSOR_MAP_SWIZZLE_128B);
-        if (rc) return rc;
-        uint64_t d3[2] = {(uint64_t)p.Ce, 25u};
-        uint64_t s3[1] = {(uint64_t)p.Ce * 2};
-        uint32_t b3[2] = {(uint32_t)FP_CB, 25u};
-        rc = make_tmap(&md, dw_cat, 2, d3, s3, b3, CU_TENSOR_MAP_SWIZZLE_NONE);
-        if (rc) return rc;
-    }
+    int rc = make_tmap_nhwc(&m0, a1, N, H, W, C1, FP_CB, FpCfg<5>::I, FpCfg<5>::I, CU_TENSOR_MAP_SWIZZLE_NONE);
+    if (rc) return rc;
+    rc = make_tmap_nhwc(&m1, a2, N, H, W, C2, FP_CB, FpCfg<5>::I, FpCfg<5>::I, CU_TENSOR_MAP_SWIZZLE_NONE);
+    if (rc) return rc;
+    rc = make_tmap_rows64(&mw, pw_packed, p.nkb * p.n_tile, 64, p.n_tile, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (rc) return rc;
+    rc = make_tmap_taps(&md, dw_cat, 25, p.Ce);
+    if (rc) return rc;
     return launch_dw_project<5, 1>(m0, m1, mw, md, p, (cudaStream_t)stream);
 }

@@ -214,20 +214,6 @@ static int set_smem_attr_once(const void* fn) {
     return LP_OK;
 }
 
-static int make_b_map(CUtensorMap* m, const void* w, int total_rows, int n_tile) {
-    uint64_t dims[2] = {(uint64_t)BK, (uint64_t)total_rows};
-    uint64_t strides[1] = {(uint64_t)BK * 2};
-    uint32_t box[2] = {(uint32_t)BK, (uint32_t)n_tile};
-    return make_tmap(m, w, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
-}
-
-static int make_act_map4(CUtensorMap* m, const void* x, int N, int H, int W, int C, int TW, int TH) {
-    uint64_t dims[4] = {(uint64_t)C, (uint64_t)W, (uint64_t)H, (uint64_t)N};
-    uint64_t strides[3] = {(uint64_t)C * 2, (uint64_t)W * C * 2, (uint64_t)H * W * C * 2};
-    uint32_t box[4] = {(uint32_t)BK, (uint32_t)TW, (uint32_t)TH, 1u};
-    return make_tmap(m, x, 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
-}
-
 static void pick_spatial_tile(int H, int W, int* TH, int* TW) {
     int best = -1, bw = 32;
     const int cands[3] = {32, 16, 8};
@@ -373,11 +359,11 @@ extern "C" int lp_fusion_deconv_f16(const void* refined, const void* raw, const 
     p.bias = bias_packed;
     p.out = out;
     CUtensorMap m0, m1, mb;
-    int rc = make_act_map4(&m0, refined, N, H, W, Cr, p.TW, p.TH);
+    int rc = make_tmap_nhwc(&m0, refined, N, H, W, Cr, BK, p.TW, p.TH, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
-    rc = make_act_map4(&m1, raw, N, H, W, Cw, p.TW, p.TH);
+    rc = make_tmap_nhwc(&m1, raw, N, H, W, Cw, BK, p.TW, p.TH, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
-    rc = make_b_map(&mb, w_packed, p.total_bt * p.n_tile, p.n_tile);
+    rc = make_tmap_rows64(&mb, w_packed, p.total_bt * p.n_tile, BK, p.n_tile, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
     return launch_gemm<MODE_DECONV>(m0, m1, mb, p, (cudaStream_t)stream);
 }
@@ -440,11 +426,11 @@ extern "C" int lp_head_pw_dual_f16(const void* a1, const void* a2, const void* w
     p.act = out_fp32 ? 1 : 0;   // MODE_HEAD reuses `act` as the output-dtype flag
     p.out = out_nchw;
     CUtensorMap m0, m1, mb;
-    int rc = make_act_map4(&m0, a1, N, H, W, C1, p.TW, p.TH);
+    int rc = make_tmap_nhwc(&m0, a1, N, H, W, C1, BK, p.TW, p.TH, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
-    rc = make_act_map4(&m1, a2, N, H, W, C2, p.TW, p.TH);
+    rc = make_tmap_nhwc(&m1, a2, N, H, W, C2, BK, p.TW, p.TH, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
-    rc = make_b_map(&mb, w_packed, p.total_bt * p.n_tile, p.n_tile);
+    rc = make_tmap_rows64(&mb, w_packed, p.total_bt * p.n_tile, BK, p.n_tile, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
     return launch_gemm<MODE_HEAD>(m0, m1, mb, p, (cudaStream_t)stream);
 }

@@ -404,10 +404,7 @@ extern "C" int lp_pw1x1_f16(const void* a, const void* w_packed, const float* bi
         if (rc) return rc;
     }
     {
-        uint64_t dims[2] = {(uint64_t)PW_BK, (uint64_t)(p.n_chunks * p.kb * p.n_tile)};
-        uint64_t strides[1] = {(uint64_t)PW_BK * 2};
-        uint32_t box[2] = {(uint32_t)PW_BK, (uint32_t)p.n_tile};
-        int rc = make_tmap(&mb, w_packed, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
+        int rc = make_tmap_rows64(&mb, w_packed, p.n_chunks * p.kb * p.n_tile, PW_BK, p.n_tile, CU_TENSOR_MAP_SWIZZLE_128B);
         if (rc) return rc;
     }
     {

@@ -132,7 +132,7 @@ stem_fused_kernel(const __grid_constant__ CUtensorMap map_w1, const __grid_const
         tma_load_2d(sm.b1, &map_w1, &sm.w_full, 0, 0);
         tma_load_2d(sm.b2, &map_w3, &sm.w_full, 0, 0);
     }
-    const __half2 zero2 = __floats2half2_rn(0.f, 0.f), six2 = __floats2half2_rn(6.f, 6.f);
+    const __half2 zero2 = __floats2half2_rn(0.f, 0.f);
 
     // image patch of the first tile -> registers
     uint4 pre[SF_PER];
@@ -226,11 +226,7 @@ stem_fused_kernel(const __grid_constant__ CUtensorMap map_w1, const __grid_const
                     for (int c = 0; c < 2; ++c) {
                         const int ch = c * 16 + frag_col(lane, i);
                         __half2 h = zero2;
-                        if (in)
-                            h = __hmin2(__hmax2(__floats2half2_rn(acc1[b][c][2 * i] + sm.bias1[ch],
-                                                                  acc1[b][c][2 * i + 1] + sm.bias1[ch + 1]),
-                                                zero2),
-                                        six2);
+                        if (in) h = expand_relu6(acc1[b][c][2 * i] + sm.bias1[ch], acc1[b][c][2 * i + 1] + sm.bias1[ch + 1]);
                         *reinterpret_cast<__half2*>(sm.t + (ch >> 3) * SF_TCHUNK + r * 16 + (ch & 7) * 2) = h;
                     }
                 }
@@ -248,6 +244,7 @@ stem_fused_kernel(const __grid_constant__ CUtensorMap map_w1, const __grid_const
             __half2 acc[4][4];
             dw_slab_hfma2<3, 4, SF_CW, 32, 4>(tile_in, reinterpret_cast<const __half2*>(&sm.wdw[0][0]), cp, mir, oy, ox, bh, acc);
             // A1 is dead (conv1 retired): the first M-tile of its buffer now holds A2 (128 pixels x 32 channels)
+            dw_relu6(acc);
             dw_store_a<4>(sm.a, 16384, acc, oy, ox, mir, cp >> 2, cp);
         }
         fence_proxy_async();
@@ -277,15 +274,9 @@ stem_fused_kernel(const __grid_constant__ CUtensorMap map_w1, const __grid_const
             for (int i = 0; i < 4; ++i) {
                 const int pix = b * 64 + frag_row(warp, lane, i);
                 const int oy = oy0 + (pix >> 4), ox = ox0 + (pix & 15);
-                if (oy < p.Ho && ox < p.Wo) {
-#pragma unroll
-                    for (int c = 0; c < 2; ++c) {
-                        const int ch = c * 16 + frag_col(lane, i);
-                        if (ch < p.C0)
-                            *reinterpret_cast<__half2*>(p.out + (((size_t)n * p.Ho + oy) * p.Wo + ox) * p.C0 + ch) =
-                                __floats2half2_rn(acc2[b][c][2 * i] + sm.biaspw[ch], acc2[b][c][2 * i + 1] + sm.biaspw[ch + 1]);
-                    }
-                }
+                if (oy < p.Ho && ox < p.Wo)
+                    proj_store_row<2>(p.out, nullptr, (((size_t)n * p.Ho + oy) * p.Wo + ox) * p.C0, p.C0, acc2[b], i, sm.biaspw,
+                                      lane);
             }
         __syncthreads();      // the A buffer, the conv1 tile and the patch are free for the next tile
     }
@@ -326,17 +317,10 @@ extern "C" int lp_stem_fused_f16(const void* x, int x_is_fp32, int flip_x, const
     p.x = x; p.b1 = b1; p.w_dw = reinterpret_cast<const __half*>(w_dw); p.b_dw = b_dw; p.b_pw = b_pw_packed;
     p.out = reinterpret_cast<__half*>(out);
     CUtensorMap m1, m3;
-    {
-        uint64_t d[2] = {64u, 32u};
-        uint64_t s[1] = {128u};
-        uint32_t b[2] = {64u, 32u};
-        int rc = make_tmap(&m1, w1_packed, 2, d, s, b, CU_TENSOR_MAP_SWIZZLE_128B);
-        if (rc) return rc;
-        uint64_t d3[2] = {64u, (uint64_t)p.n_tile};
-        uint32_t b3[2] = {64u, (uint32_t)p.n_tile};
-        rc = make_tmap(&m3, w_pw_packed, 2, d3, s, b3, CU_TENSOR_MAP_SWIZZLE_128B);
-        if (rc) return rc;
-    }
+    int rc = make_tmap_rows64(&m1, w1_packed, 32, 64, 32, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (rc) return rc;
+    rc = make_tmap_rows64(&m3, w_pw_packed, p.n_tile, 64, p.n_tile, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (rc) return rc;
     const int smem = (int)sizeof(SfSmem);      // ~58 KB: three CTAs per SM
     int grid = 3 * num_sms();
     if (grid > p.num_tiles) grid = p.num_tiles;

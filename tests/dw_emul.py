@@ -1,5 +1,6 @@
-"""Bit-exact CPU emulation of the depthwise arithmetic of lp_dwconv_f16 (dwconv.cu) and of dw_inner.cuh / the block path
-of dwpw.cu (test infrastructure, numpy only).
+"""Bit-exact CPU emulation of the depthwise arithmetic of every kernel (test infrastructure, numpy only).  It lives in one
+place on the device, dw_inner.cuh: dwconv(..., prec) restates its dw_ffma (prec 0), dw_rowsum (prec 1) and dw_hfma2
+(prec 2), which lp_dwconv_f16 (dwconv.cu), the fused block kernels (dwpw.cu, dwblock.cu), the fused stem and the heads call.
 
 Every step of the kernels' arithmetic has a unique correctly rounded result, so it can be restated exactly:
   - an fp16 x fp16 product is exact in fp32 (22 significant bits), so fp32 `x*w + acc` in numpy is the kernels' fmaf;
