@@ -20,7 +20,11 @@ EPS = 1e-5
 
 
 def _fold(sd, bn):
-    s = sd[bn + ".weight"].float() / torch.sqrt(sd[bn + ".running_var"].float() + EPS)
+    """BN (scale, shift) in fp32, every step correctly rounded: the square root is taken in fp64 and rounded once
+    to fp32, which is the correctly rounded fp32 square root.  torch's vectorised fp32 sqrt on the CPU is not always
+    (it can be one ulp off), so folding in fp32 directly would give weights that depend on the device the state_dict
+    lives on."""
+    s = sd[bn + ".weight"].float() / torch.sqrt((sd[bn + ".running_var"].float() + EPS).double()).float()
     b = sd[bn + ".bias"].float() - sd[bn + ".running_mean"].float() * s
     return s, b
 

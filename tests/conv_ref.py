@@ -10,12 +10,14 @@
                order c, ky, kx with the weights widened from fp16, clamp to [0, 6] in fp32, one RNE rounding to fp16.
   stem_im2col  the A operand of the fused stem's first GEMM (stem_fused.cu P1): [M, 32], k = c*9 + ky*3 + kx for the
                27 taps of the fp16 image, then 5 zero columns.
-  deconv_f64   ReLU(ConvT4x4s2p1(refined) + ConvT4x4s2p1(raw) + bias) in float64, with the same sum over absolute
-               values (the magnitude of the bound of gpu_util.check_bound).
+  deconv_f64   ReLU(ConvT4x4s2p1(refined) + ConvT4x4s2p1(raw) + bias) in float64, with the same sum over magnitudes
+               (fp16 subnormals lifted to 2^-14: the magnitude of the bound of gpu_util.check_bound).
   kernel selection of lp_fusion_deconv_f16 (gemm_tc.cu, deconv_rows.cu), restated from the sources."""
 import numpy as np
 import torch
 import torch.nn.functional as F
+
+from mma_emul import lift16
 
 _F64, _F32, _F16 = np.float64, np.float32, np.float16
 
@@ -87,7 +89,8 @@ def stem_im2col(x16, flip):
 # ---------------------------------------------------------------- fusion deconv
 def deconv_f64(xr, xw, wr, ww, bias):
     """xr [N,H,W,Cr], xw [N,H,W,Cw] NHWC; wr [Cr,Co,4,4], ww [Cw,Co,4,4]; bias [Co] -> (ref, mag), [N,2H,2W,Co] float64:
-    ref = ReLU(ConvT(xr, wr) + ConvT(xw, ww) + bias), mag = ConvT(|xr|, |wr|) + ConvT(|xw|, |ww|) + |bias|"""
+    ref = ReLU(ConvT(xr, wr) + ConvT(xw, ww) + bias), mag = ConvT(L(xr), L(wr)) + ConvT(L(xw), L(ww)) + |bias|,
+    L = mma_emul.lift16"""
     def t(a):
         return torch.from_numpy(np.ascontiguousarray(np.asarray(a, _F64)))
 
@@ -96,8 +99,8 @@ def deconv_f64(xr, xw, wr, ww, bias):
 
     b = t(bias).view(1, -1, 1, 1)
     ref = F.conv_transpose2d(nchw(xr), t(wr), None, 2, 1) + F.conv_transpose2d(nchw(xw), t(ww), None, 2, 1) + b
-    mag = (F.conv_transpose2d(nchw(xr).abs(), t(wr).abs(), None, 2, 1) +
-           F.conv_transpose2d(nchw(xw).abs(), t(ww).abs(), None, 2, 1) + b.abs())
+    mag = (F.conv_transpose2d(t(lift16(xr)).permute(0, 3, 1, 2), t(lift16(wr)), None, 2, 1) +
+           F.conv_transpose2d(t(lift16(xw)).permute(0, 3, 1, 2), t(lift16(ww)), None, 2, 1) + b.abs())
     return ref.clamp_min(0).permute(0, 2, 3, 1).numpy(), mag.permute(0, 2, 3, 1).numpy()
 
 

@@ -4,12 +4,14 @@ lp_pw1x1_f16 (ReLU6) -> lp_dwconv_f16 (k7, stride 2, ReLU6, packed fp16) -> lp_p
 Both expand with one wgmma per K=16 slice and round (acc + bias) to fp16 before the ReLU6, both run the depthwise chain
 of dw_inner.cuh (stride 2 has no mirrored lanes), and both project over the same K=16 slices in channel order (four per
 64-channel K block, the slices past Ce adding exact zeros) with one rounding of acc + bias.  At the LitePose shapes
-the fused output is also checked against fp64 over the emulated depthwise (dw_emul.dwconv) of the expansion."""
+the fused output is also checked against fp64 over the emulated depthwise (dw_emul.dwconv) of the expansion, and
+equal to the tensor-core emulator's projection (mma_emul.pw1x1) of that depthwise output."""
 import numpy as np
 import pytest
 import torch
 
 import dw_emul as de
+import mma_emul as me
 from litepose_b200 import _lib
 from gpu_util import check_reduction, pack_pw, stream
 
@@ -121,8 +123,10 @@ def test_block_s2_projection_fp64_over_emulated_depthwise(n, h, w, cin, ce, co):
     e = _pw(blk.xd, blk.wek2, blk.bek2, n * h * w, cin, ce, de.ACT_RELU6)
     torch.cuda.synchronize()
     d = de.dwconv(e.cpu().numpy().reshape(n, h, w, ce), wd, bd, 7, 2, de.ACT_RELU6, 2)
-    check_reduction(blk.fused().reshape(-1, co), d, wp, bp, None, ce,
-                    "block_s2 n%d %dx%d cin%d ce%d co%d" % (n, h, w, cin, ce, co))
+    fused = blk.fused().reshape(-1, co)
+    check_reduction(fused, d, wp, bp, None, ce, "block_s2 n%d %dx%d cin%d ce%d co%d" % (n, h, w, cin, ce, co))
+    assert_equal_values(fused, me.pw1x1(d.reshape(-1, ce), wp, bp),
+                        "block_s2 projection vs mma_emul n%d %dx%d cin%d ce%d co%d" % (n, h, w, cin, ce, co))
 
 
 def test_block_s2_repeated_launches_identical():

@@ -17,6 +17,7 @@ import torch
 
 import conv_ref as cr
 import dw_emul as de
+import mma_emul as me
 from litepose_b200 import _lib
 from gpu_util import check_bound, check_reduction, pack_pw, stream
 
@@ -123,6 +124,10 @@ def _check_stem_fused(n, h, w, c0, flip, seed):
     d_emul = de.dwconv(e.reshape(n, ho, wo, 32), wdw, bdw, 3, 1, de.ACT_RELU6, 2)
     assert_equal_values(d, d_emul, what + " dwconv vs dw_emul")
     check_reduction(chain, d_emul, w3, b3, None, 32, what + " 1x1")
+    # both GEMMs against the tensor-core emulator, value for value, on the first and last 16384 pixels
+    rows = np.r_[0:min(m, 16384), max(16384, m - 16384):m]
+    assert_equal_values(e[rows], me.pw1x1(a[rows], w1p[:, :32], b1, None, de.ACT_RELU6), what + " conv1 vs mma_emul")
+    assert_equal_values(chain[rows], me.pw1x1(d_emul.reshape(m, 32)[rows], w3, b3), what + " 1x1 vs mma_emul")
 
 
 @pytest.mark.parametrize("flip", [0, 1])
