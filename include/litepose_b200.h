@@ -146,7 +146,10 @@ int lp_block_s2_f16(const void* x, const void* w_exp_packed, const float* b_exp,
 /* ---- M3: fusion deconv level ----------------------------------------------
  * out = ReLU(ConvT4x4s2p1(refined) + ConvT4x4s2p1(raw) + bias), one kernel.
  * refined NHWC fp16 [N,H,W,Cr], raw [N,H,W,Cw], out [N,2H,2W,Co].
- * w_refined/w_raw: BN-scaled fp16 in the reference layout [Cin][Co][4][4] (host). */
+ * w_refined/w_raw: BN-scaled fp16 in the reference layout [Cin][Co][4][4] (host).
+ * Single branch (pose_simplenet's deconv_bnrelu(deconv_refined(refined)), no deconv_raw): Cw == 0 with
+ * w_raw / raw NULL; the K program then holds the refined channels only (row kernel: K = Cr rounded up to
+ * 16, taken for Cr <= 64).  Every Cw > 0 call and its packed layout are those of the two-branch form. */
 size_t lp_deconv_packed_elems(int Cr, int Cw, int Co);
 size_t lp_deconv_packed_bias_elems(int Co);
 int lp_deconv_pack(const uint16_t* w_refined, const uint16_t* w_raw, const float* bias, int Cr, int Cw,
@@ -158,7 +161,8 @@ int lp_fusion_deconv_f16(const void* refined, const void* raw, const void* w_pac
 /* ---- M4: head pointwise pair ------------------------------------------------
  * out_nchw[N,Co,H,W] = a1[N,H,W,C1] * W1^T + a2[N,H,W,C2] * W2^T  (no bias, no act);
  * out is fp32 (out_fp32 != 0; what the reference hands to the glue after tofp32) or fp16;
- * a1/a2 are the ReLU'd depthwise-5x5 outputs (lp_dwconv_f16).  w1 [Co][C1], w2 [Co][C2] host fp16. */
+ * a1/a2 are the ReLU'd depthwise-5x5 outputs (lp_dwconv_f16).  w1 [Co][C1], w2 [Co][C2] host fp16.
+ * Single branch: C2 == 0 with a2 / w2 NULL, out = a1 * W1^T. */
 size_t lp_head_packed_elems(int C1, int C2, int Co);
 int lp_head_pack(const uint16_t* w1, const uint16_t* w2, int C1, int C2, int Co, uint16_t* w_packed);
 int lp_head_pw_dual_f16(const void* a1, const void* a2, const void* w_packed, void* out_nchw,
@@ -169,7 +173,9 @@ int lp_head_pw_dual_f16(const void* a1, const void* a2, const void* w_packed, vo
  * (final_refined[i](refined) + final_raw[i](raw), lib/models/pose_mobilenet.py:151-154,
  * lib/models/layers/layers.py:120-133): depthwise 5x5 on the CUDA cores, result kept in shared
  * memory as the wgmma A operand, bias-free 1x1 on the tensor cores, NCHW fp32/fp16 store.
- * Pack (host memory): dw1/dw2 tap-major [25][C] BN-folded fp16 + fp32 biases, w1 [Co][C1], w2 [Co][C2]. */
+ * Pack (host memory): dw1/dw2 tap-major [25][C] BN-folded fp16 + fp32 biases, w1 [Co][C1], w2 [Co][C2].
+ * Single branch (pose_simplenet's final_refined[i](refined) alone): C2 == 0 with dw2, bdw2, w2 and a2 NULL;
+ * the slabs all come from a1 and the packed buffers carry none for the missing branch. */
 size_t lp_head_fused_dw_elems(int C1, int C2);           /* fp16 elements of dw_cat; bias: /25 fp32 */
 size_t lp_head_fused_pw_elems(int C1, int C2, int Co);   /* fp16 elements of pw_packed */
 int lp_head_fused_pack(const uint16_t* dw1, const float* bdw1, const uint16_t* dw2, const float* bdw2,

@@ -543,7 +543,8 @@ extern "C" size_t lp_head_fused_pw_elems(int C1, int C2, int Co) {
 extern "C" int lp_head_fused_pack(const uint16_t* dw1, const float* bdw1, const uint16_t* dw2, const float* bdw2,
                                   const uint16_t* w1, const uint16_t* w2, int C1, int C2, int Co, uint16_t* dw_cat,
                                   float* bdw_cat, uint16_t* pw_packed) {
-    LP_CHECK_ARG(dw1 && dw2 && w1 && w2 && dw_cat && bdw_cat && pw_packed && C1 > 0 && C2 > 0 && Co > 0,
+    // C2 == 0: single branch; with s2 == 0 no padded channel maps to the second branch, so dw2 / bdw2 / w2 are not read
+    LP_CHECK_ARG(dw1 && w1 && ((dw2 && w2) || C2 == 0) && dw_cat && bdw_cat && pw_packed && C1 > 0 && C2 >= 0 && Co > 0,
                  "lp_head_fused_pack: bad args");
     const int s1 = head_slabs(C1), s2 = head_slabs(C2), ns = s1 + s2, CP = ns * FP_CB;
     const int nt = (Co + 15) / 16 * 16, nkb = (ns + 1) / 2;
@@ -580,8 +581,8 @@ extern "C" int lp_head_fused_pack(const uint16_t* dw1, const float* bdw1, const 
 extern "C" int lp_head_fused_f16(const void* a1, const void* a2, const void* dw_cat, const float* bdw_cat,
                                  const void* pw_packed, void* out_nchw, int out_fp32, int N, int H, int W, int C1, int C2,
                                  int Co, lp_stream_t stream) {
-    LP_CHECK_ARG(a1 && a2 && dw_cat && bdw_cat && pw_packed && out_nchw, "lp_head_fused_f16: null pointer");
-    LP_CHECK_ARG(N > 0 && H > 0 && W > 0 && C1 % 8 == 0 && C2 % 8 == 0 && C1 > 0 && C2 > 0 && Co > 0 && Co <= 128,
+    LP_CHECK_ARG(a1 && (a2 || C2 == 0) && dw_cat && bdw_cat && pw_packed && out_nchw, "lp_head_fused_f16: null pointer");
+    LP_CHECK_ARG(N > 0 && H > 0 && W > 0 && C1 % 8 == 0 && C2 % 8 == 0 && C1 > 0 && C2 >= 0 && Co > 0 && Co <= 128,
                  "lp_head_fused_f16: bad shape N=%d H=%d W=%d C1=%d C2=%d Co=%d", N, H, W, C1, C2, Co);
     if ((reinterpret_cast<uintptr_t>(a1) | reinterpret_cast<uintptr_t>(a2) | reinterpret_cast<uintptr_t>(dw_cat) |
          reinterpret_cast<uintptr_t>(pw_packed)) & 15) {
@@ -607,8 +608,12 @@ extern "C" int lp_head_fused_f16(const void* a1, const void* a2, const void* dw_
     CUtensorMap m0, m1, mw, md;
     int rc = make_tmap_nhwc(&m0, a1, N, H, W, C1, FP_CB, FpCfg<5>::I, FpCfg<5>::I, CU_TENSOR_MAP_SWIZZLE_NONE);
     if (rc) return rc;
-    rc = make_tmap_nhwc(&m1, a2, N, H, W, C2, FP_CB, FpCfg<5>::I, FpCfg<5>::I, CU_TENSOR_MAP_SWIZZLE_NONE);
-    if (rc) return rc;
+    if (C2 > 0) {
+        rc = make_tmap_nhwc(&m1, a2, N, H, W, C2, FP_CB, FpCfg<5>::I, FpCfg<5>::I, CU_TENSOR_MAP_SWIZZLE_NONE);
+        if (rc) return rc;
+    } else {
+        m1 = m0;      // single branch: ns0 == nslabs, no slab is taken from map 1
+    }
     rc = make_tmap_rows64(&mw, pw_packed, p.nkb * p.n_tile, 64, p.n_tile, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
     rc = make_tmap_taps(&md, dw_cat, 25, p.Ce);

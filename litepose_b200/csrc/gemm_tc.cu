@@ -319,7 +319,8 @@ extern "C" size_t lp_deconv_packed_elems(int Cr, int Cw, int Co) {
 extern "C" size_t lp_deconv_packed_bias_elems(int Co) { return (size_t)deconv_ntile(Co); }
 extern "C" int lp_deconv_pack(const uint16_t* wr, const uint16_t* ww, const float* bias, int Cr, int Cw, int Co,
                               uint16_t* wp, float* bp) {
-    LP_CHECK_ARG(wr && ww && wp && bp, "lp_deconv_pack: null pointer");
+    // Cw == 0: single branch (no raw deconv); deconv_program and dr_pack never read w_raw then
+    LP_CHECK_ARG(wr && (ww || Cw == 0) && wp && bp, "lp_deconv_pack: null pointer");
     LP_CHECK_ARG(Cr % 8 == 0 && Cw % 8 == 0 && Co % 8 == 0 && Co <= 64, "lp_deconv_pack: bad channels %d %d %d", Cr, Cw, Co);
     int bt = 0;
     LP_CHECK_ARG(deconv_program(Cr, Cw, Co, nullptr, &bt, wr, ww, wp) > 0, "lp_deconv_pack: too many K blocks");
@@ -330,7 +331,7 @@ extern "C" int lp_deconv_pack(const uint16_t* wr, const uint16_t* ww, const floa
 
 extern "C" int lp_fusion_deconv_f16(const void* refined, const void* raw, const void* w_packed, const float* bias_packed,
                                     void* out, int N, int H, int W, int Cr, int Cw, int Co, lp_stream_t stream) {
-    LP_CHECK_ARG(refined && raw && w_packed && out, "lp_fusion_deconv_f16: null pointer");
+    LP_CHECK_ARG(refined && (raw || Cw == 0) && w_packed && out, "lp_fusion_deconv_f16: null pointer");
     LP_CHECK_ARG(N > 0 && H > 0 && W > 0 && Cr % 8 == 0 && Cw % 8 == 0 && Co % 8 == 0 && Co >= 8 && Co <= 64,
                  "lp_fusion_deconv_f16: bad shape N=%d H=%d W=%d Cr=%d Cw=%d Co=%d (Co<=64)", N, H, W, Cr, Cw, Co);
     GemmParams p;
@@ -361,8 +362,12 @@ extern "C" int lp_fusion_deconv_f16(const void* refined, const void* raw, const 
     CUtensorMap m0, m1, mb;
     int rc = make_tmap_nhwc(&m0, refined, N, H, W, Cr, BK, p.TW, p.TH, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
-    rc = make_tmap_nhwc(&m1, raw, N, H, W, Cw, BK, p.TW, p.TH, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (rc) return rc;
+    if (Cw > 0) {
+        rc = make_tmap_nhwc(&m1, raw, N, H, W, Cw, BK, p.TW, p.TH, CU_TENSOR_MAP_SWIZZLE_128B);
+        if (rc) return rc;
+    } else {
+        m1 = m0;      // single branch: no step selects map 1
+    }
     rc = make_tmap_rows64(&mb, w_packed, p.total_bt * p.n_tile, BK, p.n_tile, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
     return launch_gemm<MODE_DECONV>(m0, m1, mb, p, (cudaStream_t)stream);
@@ -373,7 +378,7 @@ extern "C" size_t lp_head_packed_elems(int C1, int C2, int Co) {
     return (size_t)((C1 + BK - 1) / BK + (C2 + BK - 1) / BK) * round_up(Co, 16) * BK;
 }
 extern "C" int lp_head_pack(const uint16_t* w1, const uint16_t* w2, int C1, int C2, int Co, uint16_t* wp) {
-    LP_CHECK_ARG(w1 && w2 && wp && C1 > 0 && C2 > 0 && Co > 0, "lp_head_pack: bad args");
+    LP_CHECK_ARG(w1 && (w2 || C2 == 0) && wp && C1 > 0 && C2 >= 0 && Co > 0, "lp_head_pack: bad args");
     const int nt = round_up(Co, 16);
     int bt = 0;
     for (int br = 0; br < 2; ++br) {
@@ -391,8 +396,8 @@ extern "C" int lp_head_pack(const uint16_t* w1, const uint16_t* w2, int C1, int 
 
 extern "C" int lp_head_pw_dual_f16(const void* a1, const void* a2, const void* w_packed, void* out_nchw, int out_fp32,
                                    int N, int H, int W, int C1, int C2, int Co, lp_stream_t stream) {
-    LP_CHECK_ARG(a1 && a2 && w_packed && out_nchw, "lp_head_pw_dual_f16: null pointer");
-    LP_CHECK_ARG(N > 0 && H > 0 && W > 0 && C1 % 8 == 0 && C2 % 8 == 0 && Co > 0 && Co <= 256,
+    LP_CHECK_ARG(a1 && (a2 || C2 == 0) && w_packed && out_nchw, "lp_head_pw_dual_f16: null pointer");
+    LP_CHECK_ARG(N > 0 && H > 0 && W > 0 && C1 % 8 == 0 && C2 % 8 == 0 && C2 >= 0 && Co > 0 && Co <= 256,
                  "lp_head_pw_dual_f16: bad shape N=%d H=%d W=%d C1=%d C2=%d Co=%d", N, H, W, C1, C2, Co);
     GemmParams p;
     memset(&p, 0, sizeof(p));
@@ -428,8 +433,12 @@ extern "C" int lp_head_pw_dual_f16(const void* a1, const void* a2, const void* w
     CUtensorMap m0, m1, mb;
     int rc = make_tmap_nhwc(&m0, a1, N, H, W, C1, BK, p.TW, p.TH, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
-    rc = make_tmap_nhwc(&m1, a2, N, H, W, C2, BK, p.TW, p.TH, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (rc) return rc;
+    if (C2 > 0) {
+        rc = make_tmap_nhwc(&m1, a2, N, H, W, C2, BK, p.TW, p.TH, CU_TENSOR_MAP_SWIZZLE_128B);
+        if (rc) return rc;
+    } else {
+        m1 = m0;      // single branch: no step selects map 1
+    }
     rc = make_tmap_rows64(&mb, w_packed, p.total_bt * p.n_tile, BK, p.n_tile, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
     return launch_gemm<MODE_HEAD>(m0, m1, mb, p, (cudaStream_t)stream);

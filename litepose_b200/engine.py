@@ -4,7 +4,9 @@
 reference lib/models/pose_mobilenet.py:21-156) into BN-folded, kernel-packed fp16
 weights (fold recipe: reference fuse_bn.py:81-137,147-162; shared-BN deconv pair:
 scale into both branches, shift once) and runs the network as a fixed sequence of
-C-ABI calls (include/litepose_b200.h) on NHWC fp16 activations.  A plan (buffers +
+C-ABI calls (include/litepose_b200.h) on NHWC fp16 activations.  The state_dict of reference
+lib/models/pose_simplenet.py (no deconv_raw.* / final_raw.*: the head without the fusion branch)
+runs the same plan with the single-branch forms of the deconv and head calls.  A plan (buffers +
 call list) is built per (N, H, W, dtype) and can be captured into a CUDA graph.
 PyTorch is used for device memory and streams only.
 """
@@ -70,6 +72,24 @@ class _Op(object):
 
 FOLDED_FORMAT = "litepose_b200-folded-1"
 
+# The two LitePose heads of the reference (named after the modules that build them): pose_mobilenet's Fusion Deconv
+# Head adds a raw branch from the backbone to every deconv level and output head; pose_simplenet, the paper's ablation
+# without it, has the same names minus deconv_raw.* / final_raw.*.
+FUSION, SIMPLE = "pose_mobilenet", "pose_simplenet"
+
+
+def _topology(sd):
+    """FUSION or SIMPLE from the state_dict's keys; a dict with the raw branch on some levels only is refused"""
+    raw = ["deconv_raw.%d.weight" % i for i in range(3)] + ["final_raw.%d.conv.3.weight" % i for i in range(2)]
+    have = [k for k in raw if k in sd]
+    if len(have) == len(raw):
+        return FUSION
+    if not have and not any(k.startswith(("deconv_raw.", "final_raw.")) for k in sd):
+        return SIMPLE
+    raise ValueError("LitePoseEngine runs the fusion head (the raw branch on all 3 deconv levels and both output heads, "
+                     "pose_mobilenet) or no raw branch at all (pose_simplenet); this state_dict has it on some levels "
+                     "only: %s present, %s missing" % (have or "no raw weights", [k for k in raw if k not in sd]))
+
 
 class LitePoseEngine(object):
     def __init__(self, state_dict, arch, device, num_joints_out=None):
@@ -111,7 +131,7 @@ class LitePoseEngine(object):
 
         walk(self.P, [])
         header = {"format": FOLDED_FORMAT, "arch": self.arch, "channels": self.channels, "meta": meta,
-                  "lib_version": int(self.lib.lp_version())}
+                  "lib_version": int(self.lib.lp_version()), "topology": self.topology}
         np.savez(path, __header__=np.frombuffer(json.dumps(header).encode(), dtype=np.uint8), **arrays)
 
     @classmethod
@@ -127,6 +147,9 @@ class LitePoseEngine(object):
             raise ValueError("folded checkpoint was packed for library version %d, this is %d (re-export it)"
                              % (header["lib_version"], int(eng.lib.lp_version())))
         eng.channels = list(header["channels"])
+        eng.topology = header.get("topology", FUSION)     # files written before the single-branch head: fusion
+        if eng.topology not in (FUSION, SIMPLE):
+            raise ValueError("folded checkpoint has an unknown head topology %r" % (eng.topology,))
         meta = header["meta"]
         root = {}
 
@@ -228,40 +251,47 @@ class LitePoseEngine(object):
         P["blocks"] = blocks
         P["deconv"] = []
         P["heads"] = []
+        self.topology = _topology(sd)
+        # single-branch head (pose_simplenet): no raw weights, Cw = C2 = 0 and NULL raw pointers in the C ABI
+        fusion = self.topology == FUSION
+
+        def addr(arr):
+            return None if arr is None else arr.ctypes.data
+
         for i in range(3):
             s, b = _fold(sd, "deconv_bnrelu.%d.0" % i)
             wr = sd["deconv_refined.%d.weight" % i].float() * s.view(1, -1, 1, 1)
-            ww = sd["deconv_raw.%d.weight" % i].float() * s.view(1, -1, 1, 1)
-            cr, cw, co = wr.shape[0], ww.shape[0], wr.shape[1]
+            ww = sd["deconv_raw.%d.weight" % i].float() * s.view(1, -1, 1, 1) if fusion else None
+            cr, cw, co = wr.shape[0], ww.shape[0] if fusion else 0, wr.shape[1]
             wp = np.zeros(self.lib.lp_deconv_packed_elems(cr, cw, co), np.uint16)
             bp = np.zeros(self.lib.lp_deconv_packed_bias_elems(co), np.float32)
             bb = np.ascontiguousarray(b.cpu().numpy())
-            a, c = _np16(wr), _np16(ww)
-            _lib.check(self.lib.lp_deconv_pack(a.ctypes.data, c.ctypes.data, bb.ctypes.data, cr, cw, co,
+            a, c = _np16(wr), _np16(ww) if fusion else None
+            _lib.check(self.lib.lp_deconv_pack(a.ctypes.data, addr(c), bb.ctypes.data, cr, cw, co,
                                                wp.ctypes.data, bp.ctypes.data), "lp_deconv_pack")
             P["deconv"].append({"w": self._dev(wp, torch.float16), "b": self._dev(bp, torch.float32),
                                 "Cr": cr, "Cw": cw, "Co": co})
             if i > 0:
                 hd = {}
-                for nm in ("final_refined", "final_raw"):
+                for nm in ("final_refined", "final_raw") if fusion else ("final_refined",):
                     p = "%s.%d.conv." % (nm, i - 1)
                     s, b = _fold(sd, p + "1")
                     hd[nm + "_dw"] = self._pack_dw(sd[p + "0.weight"].float() * s.view(-1, 1, 1, 1), b)
                 w1 = sd["final_refined.%d.conv.3.weight" % (i - 1)].float()
-                w2 = sd["final_raw.%d.conv.3.weight" % (i - 1)].float()
-                co, c1, c2 = w1.shape[0], w1.shape[1], w2.shape[1]
-                a, c = _np16(w1.reshape(co, c1)), _np16(w2.reshape(co, c2))
+                w2 = sd["final_raw.%d.conv.3.weight" % (i - 1)].float() if fusion else None
+                co, c1, c2 = w1.shape[0], w1.shape[1], w2.shape[1] if fusion else 0
+                a, c = _np16(w1.reshape(co, c1)), _np16(w2.reshape(co, c2)) if fusion else None
                 hd.update({"C1": c1, "C2": c2, "Co": co})
                 # fused head: concatenated depthwise slabs + slab-ordered 1x1 weights
-                d1, d2 = hd["final_refined_dw"], hd["final_raw_dw"]
+                d1, d2 = hd["final_refined_dw"], hd.get("final_raw_dw")
                 dwc = np.zeros(self.lib.lp_head_fused_dw_elems(c1, c2), np.uint16)
                 bdc = np.zeros(dwc.size // 25, np.float32)
                 pwc = np.zeros(self.lib.lp_head_fused_pw_elems(c1, c2, co), np.uint16)
-                x1, x2 = _np16(d1["w"].float()), _np16(d2["w"].float())
+                x1, x2 = _np16(d1["w"].float()), _np16(d2["w"].float()) if fusion else None
                 y1 = np.ascontiguousarray(d1["b"].cpu().numpy())
-                y2 = np.ascontiguousarray(d2["b"].cpu().numpy())
-                _lib.check(self.lib.lp_head_fused_pack(x1.ctypes.data, y1.ctypes.data, x2.ctypes.data, y2.ctypes.data,
-                                                       a.ctypes.data, c.ctypes.data, c1, c2, co, dwc.ctypes.data,
+                y2 = np.ascontiguousarray(d2["b"].cpu().numpy()) if fusion else None
+                _lib.check(self.lib.lp_head_fused_pack(x1.ctypes.data, y1.ctypes.data, addr(x2), addr(y2),
+                                                       a.ctypes.data, addr(c), c1, c2, co, dwc.ctypes.data,
                                                        bdc.ctypes.data, pwc.ctypes.data), "lp_head_fused_pack")
                 hd.update({"dw_cat": self._dev(dwc, torch.float16), "bdw_cat": self._dev(bdc, torch.float32),
                            "pw_cat": self._dev(pwc, torch.float16)})
@@ -360,23 +390,26 @@ class LitePoseEngine(object):
             if blk["last"]:
                 x_list.append((cur, ch, cw_))
         refined, rh, rw = x_list[-1]
-        raw = x_list[-2][0]
         outs = []
+
+        def raw_ptr(level, channels):
+            # the backbone output a raw branch reads (pose_simplenet: none, a NULL pointer with 0 channels)
+            return x_list[level][0].data_ptr() if channels else None
+
         for i in range(3):
             dc = P["deconv"][i]
             nxt = buf(n, rh * 2, rw * 2, dc["Co"])
             keep.append(nxt)
             ops.append(_Op("deconv", lib.lp_fusion_deconv_f16,
-                           [refined.data_ptr(), raw.data_ptr(), dc["w"].data_ptr(), dc["b"].data_ptr(),
+                           [refined.data_ptr(), raw_ptr(-i - 2, dc["Cw"]), dc["w"].data_ptr(), dc["b"].data_ptr(),
                             nxt.data_ptr(), n, rh, rw, dc["Cr"], dc["Cw"], dc["Co"]]))
             refined, rh, rw = nxt, rh * 2, rw * 2
-            raw = x_list[-i - 3][0]
             if i > 0:
                 hd = P["heads"][i - 1]
                 o = alloc((n, hd["Co"], rh, rw), torch.float32 if out_fp32 else f16)
                 outs.append(o)
                 ops.append(_Op("head_fused", lib.lp_head_fused_f16,
-                               [refined.data_ptr(), raw.data_ptr(), hd["dw_cat"].data_ptr(),
+                               [refined.data_ptr(), raw_ptr(-i - 3, hd["C2"]), hd["dw_cat"].data_ptr(),
                                 hd["bdw_cat"].data_ptr(), hd["pw_cat"].data_ptr(), o.data_ptr(),
                                 1 if out_fp32 else 0, n, rh, rw, hd["C1"], hd["C2"], hd["Co"]]))
         plan.update({"ops": ops, "outs": outs, "keep": keep})
