@@ -9,7 +9,7 @@ The x2 bilinear resamples are written out explicitly (SURVEY Appendix A.4:
 ``align_corners=False``; out[2m] = .25*x[m-1] + .75*x[m], out[2m+1] = .75*x[m] +
 .25*x[m+1], edge-clamped) rather than through F.interpolate, so the restatement is
 independent of the op the reference calls; other ratios fall back to the general
-rule.  Pinned against the real reference in tests/test_oracle_vs_reference.py.
+rule.  Pinned against the real reference's outputs in tests/test_oracle_golden.py.
 """
 import torch
 
