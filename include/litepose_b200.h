@@ -187,7 +187,11 @@ int lp_head_fused_f16(const void* a1, const void* a2, const void* dw_cat, const 
 
 /* ---- G1+G2: NMS (k x k window max, -inf padding) + top-K per (n,j) plane -----
  * det fp32 [N,J,H,W]; tag fp32 [N,J,H,W,T].  Order: value desc, flat index asc over
- * NMS survivors with value > 0; unused slots are (0.0f, index 0).
+ * NMS survivors with value > 0; unused slots are (0.0f, index 0).  NaN never takes a slot, and
+ * a NaN anywhere in a pixel's window suppresses it (the reference's max-pool propagates NaN).
+ * nms_kernel odd, 1..9.  Width bound (one fp32 strip buffer of at most 200 KB in shared memory):
+ * W <= 51200 / (nms_kernel + 1), e.g. 8533 at kernel 5; wider maps return LP_ERR_BAD_ARG.
+ * Any height is accepted.
  * val_k [N,J,K] f32; ind_k [N,J,K] i32 (flat y*W+x); tag_k [N,J,K,T] f32.  K <= 64.
  * min_value (double, compared as the reference does: float32 value widened to double): only survivors
  * with value > max(min_value, 0) are reported.  0 reproduces top_k as the

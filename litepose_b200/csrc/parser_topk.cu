@@ -15,6 +15,7 @@
 namespace lp {
 
 constexpr int TK_THREADS = 256;
+constexpr int TK_WARPS = TK_THREADS / 32;
 constexpr int TK_MAXK = 64;
 
 __device__ __forceinline__ unsigned long long shfl_max_u64(unsigned long long v) {
@@ -27,17 +28,27 @@ __device__ __forceinline__ unsigned long long shfl_max_u64(unsigned long long v)
 }
 
 __host__ __device__ inline int strip_rows(int W) {
-    // keep both shared planes (rows + halo) under ~96 KB
+    // keep the one staged fp32 plane (SR rows + a halo of up to 4 rows on each side) under ~96 KB
     int sr = 16;
-    while (sr > 2 && (size_t)(sr + 8) * W * 8 > 96 * 1024) sr >>= 1;
+    while (sr > 2 && (size_t)(sr + 8) * W * sizeof(float) > 96 * 1024) sr >>= 1;
     return sr;
 }
 
-constexpr int TK_SPB = 4;        // strips walked sequentially by one CTA (a "band")
+constexpr int TK_SPB = 4;            // fewest strips walked sequentially by one CTA (a "band")
+constexpr int TK_MAX_LISTS = 256;    // per-warp lists one merge warp reads: 32 lanes x 8
+
+// Strips per band: TK_SPB, or more on tall planes so that bands * TK_WARPS never exceeds TK_MAX_LISTS.
+__host__ __device__ inline int band_strips(int H, int W) {
+    const int sr = strip_rows(W);
+    const int strips = (H + sr - 1) / sr;
+    const int max_bands = TK_MAX_LISTS / TK_WARPS;
+    const int spb = (strips + max_bands - 1) / max_bands;
+    return spb > TK_SPB ? spb : TK_SPB;
+}
 
 __host__ __device__ inline int plane_bands(int H, int W) {
-    const int sr = strip_rows(W);
-    return ((H + sr - 1) / sr + TK_SPB - 1) / TK_SPB;
+    const int sr = strip_rows(W), spb = band_strips(H, W);
+    return ((H + sr - 1) / sr + spb - 1) / spb;
 }
 
 // Sorted insert of `key` into the descending list s_top[0..ntop) (capacity K <= 64) by one warp.
@@ -60,13 +71,11 @@ __device__ __forceinline__ int topk_insert(unsigned long long* s_top, int ntop, 
     return nnew;
 }
 
-constexpr int TK_WARPS = TK_THREADS / 32;
-
 // Geometry of one (image, joint) plane.  Uniform call (desc == nullptr): every plane is H x W, planes are adjacent, the
 // per-warp candidate lists of plane p start at p * nbands * TK_WARPS * K.  Ragged call: image n = plane / J has its own
 // size and det / tag offsets (desc[n]); its lists follow those of images 0..n-1 (prefix sum over the images).
 struct PlaneGeom {
-    int H, W, SR, nbands;
+    int H, W, SR, spb, nbands;
     size_t det_off, tag_off, list_off;
 };
 
@@ -76,6 +85,7 @@ __device__ __forceinline__ PlaneGeom plane_geom(const lp_map_desc_t* desc, int p
         g.H = H;
         g.W = W;
         g.SR = strip_rows(W);
+        g.spb = band_strips(H, W);
         g.nbands = plane_bands(H, W);
         g.det_off = (size_t)plane * H * W;
         g.tag_off = (size_t)plane * H * W * T;
@@ -88,6 +98,7 @@ __device__ __forceinline__ PlaneGeom plane_geom(const lp_map_desc_t* desc, int p
     g.H = desc[n].h;
     g.W = desc[n].w;
     g.SR = strip_rows(g.W);
+    g.spb = band_strips(g.H, g.W);
     g.nbands = plane_bands(g.H, g.W);
     g.det_off = (size_t)desc[n].det_offset + (size_t)j * g.H * g.W;
     g.tag_off = (size_t)desc[n].tag_offset + (size_t)j * g.H * g.W * T;
@@ -96,7 +107,7 @@ __device__ __forceinline__ PlaneGeom plane_geom(const lp_map_desc_t* desc, int p
 }
 
 // partial: per plane [bands * TK_WARPS][K] keys (PlaneGeom::list_off) (sorted, 0 = empty); plane_thr: [N*J] running lower bound of the plane's
-// K-th key (zero-initialised by the caller).  One CTA walks TK_SPB strips of SR rows of one plane; inside a strip every
+// K-th key (zero-initialised by the caller).  One CTA walks PlaneGeom::spb strips of SR rows of one plane; inside a strip every
 // warp owns the rows r == warp (mod 8) and keeps its OWN sorted top-K list (no block barriers, no serial merge).  A pixel
 // can only matter if its key reaches the best known K-th key -- the maximum over all warps of the CTA (shared memory)
 // and over all CTAs of the plane (global memory) of their local K-th keys, each a valid lower bound of the plane's
@@ -124,8 +135,8 @@ nms_topk_strip_kernel(const float* __restrict__ det, const lp_map_desc_t* __rest
     unsigned long long* mytop = s_top[warp];
     const bool vec = (W & 3) == 0 && ((reinterpret_cast<uintptr_t>(p) & 15) == 0);
 
-    for (int st = 0; st < TK_SPB; ++st) {
-        const int y0 = (band * TK_SPB + st) * SR;
+    for (int st = 0; st < geo.spb; ++st) {
+        const int y0 = (band * geo.spb + st) * SR;
         if (y0 >= H) break;
         const int rows = min(SR, H - y0);
         const int hrows = rows + 2 * R;
@@ -169,11 +180,17 @@ nms_topk_strip_kernel(const float* __restrict__ det, const lp_map_desc_t* __rest
             // cheap reject first: most pixels lose against a direct neighbour
             const float l = x > 0 ? c[-1] : NEG_INF, rr = x < W - 1 ? c[1] : NEG_INF;
             if (R > 0 && !(v >= l && v >= rr && v >= c[-W] && v >= c[W])) return 0ull;
+            // the reference's max-pool propagates NaN: a NaN anywhere in the window suppresses the peak
             float m = NEG_INF;
+            bool nan = false;
             const int xa = max(x - R, 0), xb = min(x + R, W - 1);
             for (int d = 0; d <= 2 * R; ++d)
-                for (int xx = xa; xx <= xb; ++xx) m = fmaxf(m, s_val[(r + d) * W + xx]);
-            if (v != m) return 0ull;
+                for (int xx = xa; xx <= xb; ++xx) {
+                    const float s = s_val[(r + d) * W + xx];
+                    nan |= s != s;
+                    m = fmaxf(m, s);
+                }
+            if (nan || v != m) return 0ull;
             const unsigned idx = (unsigned)((y0 + r) * W + x);
             return ((unsigned long long)__float_as_uint(v) << 32) | (0xffffffffu - idx);
         };
@@ -255,7 +272,7 @@ topk_merge_kernel(const unsigned long long* __restrict__ partial, const float* _
     const unsigned long long* pl = partial + geo.list_off;
     const float* tg = tag + geo.tag_off;
     // each lane owns strips lane, lane+32, ...; head[] = cursor into each sorted strip list
-    constexpr int MAXS = 8;   // up to 256 strips
+    constexpr int MAXS = TK_MAX_LISTS / 32;
     int head[MAXS];
 #pragma unroll
     for (int i = 0; i < MAXS; ++i) head[i] = 0;
@@ -327,9 +344,9 @@ static int topk_launch(const float* det, const float* tag, int N, const int32_t*
         const int h = hw_host ? hw_host[2 * n] : H, w = hw_host ? hw_host[2 * n + 1] : W;
         LP_CHECK_ARG(h > 0 && w > 0 && (long long)h * w < (1ll << 31), "%s: bad map size %dx%d (image %d)", name, h, w, n);
         const int nb = plane_bands(h, w);
-        LP_CHECK_ARG(nb * TK_WARPS <= 256, "%s: plane too large (H=%d W=%d)", name, h, w);
         const size_t sm = (size_t)(strip_rows(w) + 2 * R) * w * sizeof(float);
-        LP_CHECK_ARG(sm <= 200 * 1024, "%s: W=%d too wide for the strip buffers", name, w);
+        // the strip buffer bounds the width: W <= 51200 / (nms_kernel + 1) (include/litepose_b200.h)
+        LP_CHECK_ARG(sm <= 200 * 1024, "%s: W=%d too wide for the strip buffers (NMS kernel %d)", name, w, nms_kernel);
         max_bands = nb > max_bands ? nb : max_bands;
         smem = sm > smem ? sm : smem;
     }

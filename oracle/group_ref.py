@@ -14,7 +14,9 @@ choice because the reference delegates to implementation-defined behaviour:
     taken over NMS survivors with value > 0; if fewer than K such survivors exist
     the remaining slots are (val 0.0, flat index 0).  Slots with val <= 0 can never
     pass ``val > DETECTION_THRESHOLD`` (threshold >= 0 is asserted), so they do not
-    influence grouping.
+    influence grouping.  NaN never takes a slot (``torch.topk`` would rank it
+    first): ``nms`` propagates NaN like the reference's max-pool, so a NaN pixel
+    and every pixel with a NaN in its window drop out at ``> 0``.
   * ``py_max_match`` (group.py:19-23) calls the third-party ``munkres`` package;
     see oracle/munkres_ref.py ("parity unpinned" at that boundary).
 
@@ -46,15 +48,22 @@ class Params(object):
                                 [1, 2, 3, 4, 5, 6, 7, 12, 13, 8, 9, 10, 11, 14, 15, 16, 17]]
 
 
-def py_max_match(scores):
+def py_max_match(scores, solver=Munkres):
     """group.py:19-23."""
-    return np.array(Munkres().compute(scores)).astype(np.int32)
+    return np.array(solver().compute(scores)).astype(np.int32)
 
 
-def match_by_tag(inp, params):
+def match_by_tag(inp, params, solver=Munkres, events=None):
     """group.py:26-97, statement by statement (float64 joints rows, float32 running
     tag means via np.mean, round-half-even cost, 1e10 column padding, dict keyed by
-    the float32 tag[0] in insertion order)."""
+    the float32 tag[0] in insertion order).  ``solver`` and ``events`` (a
+    collections.Counter) let the edge tests count which branches a case reaches;
+    neither changes the result."""
+    ev = events if events is not None else {}
+
+    def hit(name, cond=True):
+        if cond:
+            ev[name] = ev.get(name, 0) + 1
     tag_k, loc_k, val_k = inp
     default_ = np.zeros((params.num_joints, 3 + tag_k.shape[2]))
     joint_dict = {}
@@ -71,24 +80,30 @@ def match_by_tag(inp, params):
         if i == 0 or len(joint_dict) == 0:
             for tag, joint in zip(tags, joints):
                 key = tag[0]
+                hit("key_collision", key in joint_dict)
                 joint_dict.setdefault(key, np.copy(default_))[idx] = joint
                 tag_dict[key] = [tag]
         else:
             grouped_keys = list(joint_dict.keys())[:params.max_num_people]
             grouped_tags = [np.mean(tag_dict[k], axis=0) for k in grouped_keys]
             if params.ignore_too_much and len(grouped_keys) == params.max_num_people:
+                hit("ignore_too_much_skip")
                 continue
             diff = joints[:, None, 3:] - np.array(grouped_tags)[None, :, :]
             diff_normed = np.linalg.norm(diff, ord=2, axis=2)
             diff_saved = np.copy(diff_normed)
+            hit("dist_eq_threshold", bool((diff_saved == params.tag_threshold).any()))
             if params.use_detection_val:
+                hit("round_half_tie", bool((np.abs(diff_normed - np.floor(diff_normed) - 0.5) == 0).any()))
                 diff_normed = np.round(diff_normed) * 100 - joints[:, 2:3]
             num_added = diff.shape[0]
             num_grouped = diff.shape[1]
+            hit("pad_rows", num_added < num_grouped)
+            hit("pad_cols", num_added > num_grouped)
             if num_added > num_grouped:
                 diff_normed = np.concatenate(
                     (diff_normed, np.zeros((num_added, num_added - num_grouped)) + 1e10), axis=1)
-            pairs = py_max_match(diff_normed)
+            pairs = py_max_match(diff_normed, solver)
             for row, col in pairs:
                 if row < num_added and col < num_grouped and diff_saved[row][col] < params.tag_threshold:
                     key = grouped_keys[col]
@@ -96,6 +111,7 @@ def match_by_tag(inp, params):
                     tag_dict[key].append(tags[row])
                 else:
                     key = tags[row][0]
+                    hit("key_collision", key in joint_dict)
                     joint_dict.setdefault(key, np.copy(default_))[idx] = joints[row]
                     tag_dict[key] = [tags[row]]
     return np.array([joint_dict[k] for k in joint_dict]).astype(np.float32)

@@ -44,9 +44,26 @@ def test_parser_golden(golden_dir, case):
         assert np.array_equal(np.asarray(scores, np.float32), z["scores_a%d_r%d" % (adj, ref)])
 
 
-@pytest.mark.parametrize("h,w,t,people", [(64, 64, 2, 4), (96, 160, 1, 9), (200, 120, 2, 20)])
-def test_parser_batch_vs_oracle(h, w, t, people):
+# the config knobs HeatmapParser hands to the kernels, each away from its shipped value
+KNOBS = {
+    "nodetval": {"USE_DETECTION_VAL": False},
+    "ignore": {"IGNORE_TOO_MUCH": True, "MAX_NUM_PEOPLE": 8},
+    "nms3": {"NMS_KERNEL": 3, "NMS_PADDING": 1},
+    "nms7": {"NMS_KERNEL": 7, "NMS_PADDING": 3},
+    "tagthr05": {"TAG_THRESHOLD": 0.5},
+    "detthr02": {"DETECTION_THRESHOLD": 0.2},
+}
+BATCH_CASES = [pytest.param(64, 64, 2, 4, None, id="64-64-2-4"), pytest.param(96, 160, 1, 9, None, id="96-160-1-9"),
+               pytest.param(200, 120, 2, 20, None, id="200-120-2-20")]
+BATCH_CASES += [pytest.param(h, w, t, p, k, id="%d-%d-%d-%d-%s" % (h, w, t, p, k))
+                for k in KNOBS for h, w, t, p in [(96, 160, 1, 9), (200, 120, 2, 20)]]
+
+
+@pytest.mark.parametrize("h,w,t,people,knob", BATCH_CASES)
+def test_parser_batch_vs_oracle(h, w, t, people, knob):
     cfg = get_cfg(input_size=256)
+    for key, v in KNOBS.get(knob, {}).items():
+        setattr(cfg.DATASET if key == "MAX_NUM_PEOPLE" else cfg.TEST, key, v)
     n = 5
     det, tag = synth.plant_crowd_batch(n, 14, h, w, t, num_people=people, seed=100)
     det[3] = np.random.RandomState(1).uniform(0, 0.02, det[3].shape).astype(np.float32)   # an image with nobody
@@ -163,7 +180,8 @@ def test_glue_nonsquare_projection():
 
 
 def test_topk_dense_fallback():
-    """more than 2048 NMS survivors in one strip (large plateau) takes the dense-scan path"""
+    """a whole-plane plateau (every pixel survives the NMS, the K slots are the first K indices) and a plateau over
+    most of a plane broken by one higher peak"""
     cfg = get_cfg(input_size=256)
     rng = np.random.RandomState(4)
     det = rng.uniform(0, 0.02, (1, 14, 64, 160)).astype(np.float32)
