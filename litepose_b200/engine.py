@@ -92,10 +92,14 @@ def _topology(sd):
 
 
 class LitePoseEngine(object):
-    def __init__(self, state_dict, arch, device, num_joints_out=None):
+    def __init__(self, state_dict, arch, device, num_joints_out=None, residual=None, strides=None):
+        """``residual`` / ``strides``: per inverted-residual block, stage-major, whether it adds its input and its
+        stride.  By default a block's stride is its stage's on block 0 and 1 after, and it adds its input when the
+        stride is 1 and its widths are equal (LitePose's rule); the super-network fixes both by its own structure
+        (litepose_b200.subnet.derive_supernet_subnet)."""
         self._init_common(arch, device)
         sd = {k: v.detach() for k, v in state_dict.items()}
-        self._prep(sd)
+        self._prep(sd, residual, strides)
 
     def _init_common(self, arch, device):
         """device 'cpu' is accepted for weight preparation / folded-checkpoint conversion only: run() needs CUDA."""
@@ -201,8 +205,12 @@ class LitePoseEngine(object):
         wt = w.reshape(c, k * k).t().contiguous()   # tap-major [k*k][C]
         return {"w": wt.half().to(self.device), "b": bias.float().contiguous().to(self.device), "C": c, "k": k}
 
-    def _prep(self, sd):
+    def _prep(self, sd, residual=None, strides=None):
         arch = self.arch
+        total = sum(st["num_blocks"] for st in arch["backbone_setting"])
+        for name, per_block in (("residual", residual), ("strides", strides)):
+            if per_block is not None and len(per_block) != total:
+                raise ValueError("%s lists %d blocks, the architecture has %d" % (name, len(per_block), total))
         P = {}
         n_dec = len([k for k in sd if k.startswith("deconv_refined.") and k.endswith(".weight")])
         if n_dec != 3 or tuple(sd["first.0.0.weight"].shape) != (32, 3, 3, 3):
@@ -226,7 +234,7 @@ class LitePoseEngine(object):
         for si, st in enumerate(arch["backbone_setting"]):
             for bi in range(st["num_blocks"]):
                 p = "stage.%d.%d." % (si, bi)
-                stride = st["stride"] if bi == 0 else 1
+                stride = int(strides[len(blocks)]) if strides is not None else st["stride"] if bi == 0 else 1
                 s, b = _fold(sd, p + "inv.1")
                 inv = self._pack_pw(sd[p + "inv.0.weight"].float() * s.view(-1, 1, 1, 1), b)
                 s, b = _fold(sd, p + "depth_conv.1")
@@ -234,6 +242,10 @@ class LitePoseEngine(object):
                 s, b = _fold(sd, p + "point_conv.1")
                 pc = self._pack_pw(sd[p + "point_conv.0.weight"].float() * s.view(-1, 1, 1, 1), b)
                 cin, cout = inv["K"], pc["N"]
+                res = stride == 1 and cin == cout if residual is None else bool(residual[len(blocks)])
+                if res and (stride != 1 or cin != cout):
+                    raise ValueError("%s: an identity add needs stride 1 and equal widths, the block has stride %d "
+                                     "and %d -> %d channels" % (p[:-1], stride, cin, cout))
                 if dw["k"] == 7 and ((stride == 1 and self.lib.lp_block_s1_supported(cin, inv["N"], cout)) or
                                      (stride == 2 and self.lib.lp_block_s2_supported(cin, inv["N"], cout))):
                     # block-fused kernel (lp_block_s1_f16 / lp_block_s2_f16): expansion weights as [Ce][Cin padded to
@@ -246,7 +258,7 @@ class LitePoseEngine(object):
                     inv["wblk"] = self._dev(wk, torch.float16)
                     inv["bblk"] = _fold(sd, p + "inv.1")[1].float().contiguous().to(self.device)
                 blocks.append({"inv": inv, "dw": dw, "pc": pc, "stride": stride, "stage": si,
-                               "res": stride == 1 and cin == cout, "last": bi == st["num_blocks"] - 1})
+                               "res": res, "last": bi == st["num_blocks"] - 1})
             self.channels.append(blocks[-1]["pc"]["N"])
         P["blocks"] = blocks
         P["deconv"] = []

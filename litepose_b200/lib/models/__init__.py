@@ -1,15 +1,15 @@
 """Drop-in for the reference's ``models`` package (reference lib/models/__init__.py).
 
 Put ``<repo>/litepose_b200/lib`` in front of ``<reference>/lib`` on ``sys.path``:
-``models.pose_mobilenet`` and ``models.pose_simplenet`` (what valid.py:130 resolves for
-MODEL.NAME pose_mobilenet / pose_simplenet) are the sm_90a-backed modules of this repo;
+``models.pose_mobilenet``, ``models.pose_simplenet`` and ``models.pose_supermobilenet`` (what valid.py:130
+resolves for MODEL.NAME pose_mobilenet / pose_simplenet / pose_supermobilenet) are the sm_90a-backed modules of this repo;
 every other ``models.<name>`` is resolved lazily from the reference tree found further
 down ``sys.path`` (out-of-scope model zoo)."""
 import importlib
 import os
 import sys
 
-from . import pose_mobilenet, pose_simplenet  # noqa: F401
+from . import pose_mobilenet, pose_simplenet, pose_supermobilenet  # noqa: F401
 
 _here = os.path.dirname(os.path.abspath(__file__))
 try:

@@ -92,23 +92,35 @@ class EngineModule(nn.Module):
             out[k] = obj
         return out
 
-    def lp_engine(self, device=None):
-        from litepose_b200.engine import LitePoseEngine
+    def _lp_device_key(self, device):
         dev = torch.device(device) if device is not None else next(self.parameters()).device
         if dev.type != "cuda":
             raise RuntimeError("the litepose_b200 engine needs the module on a CUDA device")
-        key = (dev.type, dev.index if dev.index is not None else torch.cuda.current_device())
+        return (dev.type, dev.index if dev.index is not None else torch.cuda.current_device())
+
+    def _lp_cached(self, key, build, capacity=None):
+        """The engine cached under ``key`` while the module's weights are those it was built from, else
+        ``build(state_dict, device)``.  ``capacity``: keep at most that many engines, least recently used dropped."""
         # DataParallel replicas receive freshly broadcast tensors on every forward (version 0, new identity): they use
         # the signature the master published when it was replicated
         replica = getattr(self, "_is_replica", False)
         sig = self._lp_cache.master_sig if replica else self._lp_signature()
         with self._lp_cache.lock:
-            hit = self._lp_cache.engines.get(key)
+            engines = self._lp_cache.engines
+            hit = engines.pop(key, None)
             if hit is not None and hit[1] == sig:
+                engines[key] = hit              # most recently used last
                 return hit[0]
-            eng = LitePoseEngine(self._lp_state(), self.cfg_arch, torch.device("cuda", key[1]))
-            self._lp_cache.engines[key] = (eng, sig)
+            eng = build(self._lp_state(), torch.device("cuda", key[1]))
+            engines[key] = (eng, sig)
+            while capacity is not None and len(engines) > capacity:
+                del engines[next(iter(engines))]
             return eng
+
+    def lp_engine(self, device=None):
+        from litepose_b200.engine import LitePoseEngine
+        key = self._lp_device_key(device)
+        return self._lp_cached(key, lambda state, dev: LitePoseEngine(state, self.cfg_arch, dev))
 
     def forward(self, x):
         if x.is_cuda and not self.training:
