@@ -10,6 +10,8 @@
  *                        <- InvBottleneck.forward     lib/models/layers/layers.py:90-118
  *   lp_fusion_deconv_*   <- deconv_refined/raw + BN + ReLU
  *                                                     lib/models/pose_mobilenet.py:102-135,146-149
+ *   lp_bn_*              <- train-mode BatchNorm2d (the super-network's BN recalibration,
+ *                           calibrate_test.py:58-61; lib/models/layers/super_layers.py:19-28)
  *   lp_head_*            <- final_refined/final_raw (SepConv2d)
  *                                                     lib/models/pose_mobilenet.py:86-100,151-154
  *                                                     lib/models/layers/layers.py:120-133
@@ -72,6 +74,10 @@ void lp_reset_launch_count(void);
  * torch.flip(x, [3]) (the flip-test pass, lib/core/inference.py:120) without a copy. */
 int lp_stem_conv3x3_s2(const void* x, int x_is_fp32, int flip_x, const void* w, const float* bias,
                        void* y, int N, int H, int W, lp_stream_t stream);
+/* The same with the activation chosen: act LP_ACT_RELU6 (lp_stem_conv3x3_s2) or LP_ACT_NONE (bias may be NULL: the
+ * raw convolution, rounded once to fp16, that the BN recalibration pass takes batch statistics of). */
+int lp_stem_conv3x3_s2_act(const void* x, int x_is_fp32, int flip_x, const void* w, const float* bias,
+                           void* y, int N, int H, int W, int act, lp_stream_t stream);
 
 /* ---- M1 fused: the whole stem (conv3x3 s2 + BN + ReLU6 -> dw3x3 + BN + ReLU6 -> 1x1 + BN) in ONE kernel ----------
  * reference lib/models/pose_mobilenet.py:36-41.  x NCHW fp32/fp16 as above (flip_x = mirrored pass); w1_packed [32][64]
@@ -157,6 +163,29 @@ int lp_deconv_pack(const uint16_t* w_refined, const uint16_t* w_raw, const float
 int lp_fusion_deconv_f16(const void* refined, const void* raw, const void* w_packed,
                          const float* bias_packed, void* out, int N, int H, int W, int Cr, int Cw,
                          int Co, lp_stream_t stream);
+/* The same with the activation chosen: act LP_ACT_RELU (lp_fusion_deconv_f16) or LP_ACT_NONE (the raw sum of both
+ * branches + bias, for the BN recalibration pass).  Same kernel selection and accumulation order. */
+int lp_fusion_deconv_act_f16(const void* refined, const void* raw, const void* w_packed,
+                             const float* bias_packed, void* out, int N, int H, int W, int Cr, int Cw,
+                             int Co, int act, lp_stream_t stream);
+
+/* ---- train-mode BatchNorm (BN recalibration) -------------------------------
+ * lp_bn_stats_f16: batch statistics of x NHWC fp16 [M, C] (M = N*H*W pixels) and, per channel c,
+ *   scale[c] = gamma / sqrt(var + eps), shift[c] = beta - mean * scale (var the biased variance),
+ *   new_mean[c] = (1 - momentum) * running_mean + momentum * mean,
+ *   new_var[c]  = (1 - momentum) * running_var + momentum * var * M / (M - 1);
+ * sets *nonfinite = 1 (and leaves it otherwise) when one of those values is not finite.  gamma, beta, running_*, scale,
+ * shift, new_* fp32 [C].  Sums in fp64 over fixed pixel ranges, merged in a fixed order (bn_train.cu states it): the
+ * result is the same bits on every run.  M >= 2, C % 8 == 0; workspace of lp_bn_stats_workspace_bytes(M, C) bytes,
+ * x and workspace 16-byte aligned.
+ * lp_bn_apply_f16: y = act(fmaf(x, scale, shift)) (+ residual) in fp32, one rounding to fp16; x, residual, y [M, C];
+ * y may be x.  ReLU maps v to (v > 0 ? v : +0), ReLU6 then to min(v, 6).  C % 8 == 0, 16-byte aligned pointers. */
+size_t lp_bn_stats_workspace_bytes(int M, int C);
+int lp_bn_stats_f16(const void* x, int M, int C, const float* gamma, const float* beta, const float* running_mean,
+                    const float* running_var, double momentum, double eps, float* scale, float* shift, float* new_mean,
+                    float* new_var, int* nonfinite, void* workspace, size_t workspace_bytes, lp_stream_t stream);
+int lp_bn_apply_f16(const void* x, const float* scale, const float* shift, const void* residual, void* y, int M, int C,
+                    int act, lp_stream_t stream);
 
 /* ---- M4: head pointwise pair ------------------------------------------------
  * out_nchw[N,Co,H,W] = a1[N,H,W,C1] * W1^T + a2[N,H,W,C2] * W2^T  (no bias, no act);

@@ -35,6 +35,7 @@ SIGNATURES = {
     "lp_launch_count": (_c.c_uint64, []),
     "lp_reset_launch_count": (None, []),
     "lp_stem_conv3x3_s2": (_i, [_vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "lp_stem_conv3x3_s2_act": (_i, [_vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "lp_stem_fused_supported": (_i, [_i, _i, _i]),
     "lp_stem_fused_f16": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "lp_dwconv_f16": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
@@ -55,6 +56,10 @@ SIGNATURES = {
     "lp_deconv_packed_bias_elems": (_sz, [_i]),
     "lp_deconv_pack": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp]),
     "lp_fusion_deconv_f16": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
+    "lp_fusion_deconv_act_f16": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "lp_bn_stats_workspace_bytes": (_sz, [_i, _i]),
+    "lp_bn_stats_f16": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _d, _d, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "lp_bn_apply_f16": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "lp_head_packed_elems": (_sz, [_i, _i, _i]),
     "lp_head_pack": (_i, [_vp, _vp, _i, _i, _i, _vp]),
     "lp_head_pw_dual_f16": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),

@@ -403,5 +403,12 @@ __device__ __forceinline__ float act_apply(float v, int act) {
     return v;
 }
 
+// Fusion-deconv epilogue activation (both deconv kernels): ReLU in the network, none for the raw sums the BN
+// recalibration pass takes its batch statistics of.
+template <int ACT>
+__device__ __forceinline__ float deconv_act(float v) {
+    return ACT == LP_ACT_RELU ? fmaxf(v, 0.f) : v;
+}
+
 #endif  // __CUDACC__
 }  // namespace lp

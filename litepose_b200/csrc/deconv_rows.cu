@@ -13,8 +13,8 @@
 //                   slot (the 128B swizzle is a function of the absolute shared-memory address, so a row-shifted view
 //                   stays consistent); the weights of all 16 (tap, phase) sub-tiles stay resident in shared memory;
 //                   the 4 phase accumulators (fp32, <= 256 columns) live in registers.  Epilogue from the accumulator
-//                   fragments: bias + ReLU, fp16, staged in shared memory so that each of the two output rows of the
-//                   tile leaves as fully contiguous 16-byte stores
+//                   fragments: bias + ReLU (ACT: none for the BN recalibration pass), fp16, staged in shared memory so
+//                   that each of the two output rows of the tile leaves as fully contiguous 16-byte stores
 #include "common.cuh"
 
 namespace lp {
@@ -104,7 +104,7 @@ __device__ __forceinline__ void dr_mma_tile(float (&acc)[4 * NCH][8], const uint
     }
 }
 
-template <int NCH>
+template <int NCH, int ACT>
 __global__ void __launch_bounds__(DR_THREADS, 1)
 deconv_rows_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__ DrParams p) {
     extern __shared__ __align__(1024) uint8_t smem[];
@@ -256,7 +256,7 @@ deconv_rows_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_consta
                     const int co = (c - pos * NCH) * 16 + frag_col(lane, i);
                     if (co < Co)
                         *reinterpret_cast<__half2*>(st + a * (DR_TW * p.pair_pitch) + px * p.pair_pitch + b * (Co * 2) + co * 2) =
-                            __floats2half2_rn(fmaxf(acc[c][2 * i] + sBias[co], 0.f), fmaxf(acc[c][2 * i + 1] + sBias[co + 1], 0.f));
+                            __floats2half2_rn(deconv_act<ACT>(acc[c][2 * i] + sBias[co]), deconv_act<ACT>(acc[c][2 * i + 1] + sBias[co + 1]));
                 }
             }
             asm volatile("bar.sync 1, 256;" ::: "memory");
@@ -336,8 +336,9 @@ void deconv_rows_pack(const uint16_t* wr, const uint16_t* ww, int Cr, int Cw, in
 // the row kernel pays off on wide maps (a strip is 128 pixels); narrow levels keep the tiled kernel
 bool deconv_rows_shape_ok(int W) { return W >= 64; }
 
-int launch_deconv_rows(const void* refined, const void* raw, const void* w_rows, const float* bias_packed, void* out, int N,
-                       int H, int W, int Cr, int Cw, int Co, cudaStream_t stream) {
+template <int ACT>
+static int launch_deconv_rows_act(const void* refined, const void* raw, const void* w_rows, const float* bias_packed,
+                                  void* out, int N, int H, int W, int Cr, int Cw, int Co, cudaStream_t stream) {
     DrParams p;
     memset(&p, 0, sizeof(p));
     p.refined = reinterpret_cast<const __half*>(refined);
@@ -360,8 +361,8 @@ int launch_deconv_rows(const void* refined, const void* raw, const void* w_rows,
     }
     const size_t smem = dr_smem_bytes(Co);
     // accumulator width: 4 phases x n_tile columns, 16 per chunk
-    auto kern = p.n_tile <= 16 ? deconv_rows_kernel<1> : p.n_tile <= 32 ? deconv_rows_kernel<2>
-              : p.n_tile <= 48 ? deconv_rows_kernel<3> : deconv_rows_kernel<4>;
+    auto kern = p.n_tile <= 16 ? deconv_rows_kernel<1, ACT> : p.n_tile <= 32 ? deconv_rows_kernel<2, ACT>
+              : p.n_tile <= 48 ? deconv_rows_kernel<3, ACT> : deconv_rows_kernel<4, ACT>;
     cudaError_t e = cudaFuncSetAttribute((const void*)kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(deconv_rows)");
     int grid = p.items < num_sms() ? p.items : num_sms();
@@ -369,6 +370,12 @@ int launch_deconv_rows(const void* refined, const void* raw, const void* w_rows,
     if (le != cudaSuccess) return cuda_fail(le, "launch deconv_rows_kernel");
     LP_LAUNCH_CHECK("deconv_rows_kernel");
     return LP_OK;
+}
+
+int launch_deconv_rows(const void* refined, const void* raw, const void* w_rows, const float* bias_packed, void* out, int N,
+                       int H, int W, int Cr, int Cw, int Co, int act, cudaStream_t stream) {
+    return act == LP_ACT_RELU ? launch_deconv_rows_act<LP_ACT_RELU>(refined, raw, w_rows, bias_packed, out, N, H, W, Cr, Cw, Co, stream)
+                              : launch_deconv_rows_act<LP_ACT_NONE>(refined, raw, w_rows, bias_packed, out, N, H, W, Cr, Cw, Co, stream);
 }
 
 }  // namespace lp

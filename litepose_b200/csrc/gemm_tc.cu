@@ -4,7 +4,8 @@
 // One persistent, warp-specialised kernel covers the two spatial contractions of the network
 // (reference lib/models/pose_mobilenet.py:102-154):
 //   MODE_DECONV fusion deconv level: 4 sub-pixel phases, each a K = 4*(Cr+Cw) contraction, both branches,
-//               folded-BN bias + ReLU, written interleaved into the 2x up-sampled NHWC output
+//               folded-BN bias + ReLU (ACT: none for the BN recalibration pass), written interleaved into the
+//               2x up-sampled NHWC output
 //   MODE_HEAD   head pair:  out_nchw_f32 = A1 W1^T + A2 W2^T
 //
 // Structure per CTA (384 threads, 1 CTA/SM, grid = min(#tiles, #SMs)):
@@ -65,7 +66,7 @@ struct __align__(8) GemmBarriers {
 
 constexpr size_t GEMM_SMEM = 1024 /*align slack*/ + (size_t)STAGES * (A_BYTES + B_BYTES) + MAX_BIAS * 4 + 256;
 
-template <int MODE>
+template <int MODE, int ACT>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUtensorMap mapA1,
                const __grid_constant__ CUtensorMap mapB, const __grid_constant__ GemmParams p) {
@@ -175,8 +176,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
                                 const int a = ph >> 1, b = ph & 1;
                                 __half* op = out + ((((long long)n * 2 * p.H + 2 * y + a) * (2 * p.W)) + 2 * x + b) * Co + co;
                                 *reinterpret_cast<__half2*>(op) =
-                                    __floats2half2_rn(fmaxf(acc[c][2 * i] + sBias[co], 0.f),
-                                                      fmaxf(acc[c][2 * i + 1] + sBias[co + 1], 0.f));
+                                    __floats2half2_rn(deconv_act<ACT>(acc[c][2 * i] + sBias[co]),
+                                                      deconv_act<ACT>(acc[c][2 * i + 1] + sBias[co + 1]));
                             }
                         }
                     }
@@ -226,14 +227,14 @@ static void pick_spatial_tile(int H, int W, int* TH, int* TW) {
     *TH = BM / bw;
 }
 
-template <int MODE>
+template <int MODE, int ACT = LP_ACT_NONE>
 static int launch_gemm(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const GemmParams& p,
                        cudaStream_t stream) {
-    int rc = set_smem_attr_once((const void*)gemm_tc_kernel<MODE>);
+    int rc = set_smem_attr_once((const void*)gemm_tc_kernel<MODE, ACT>);
     if (rc) return rc;
     const int grid = p.num_tiles < num_sms() ? p.num_tiles : num_sms();
     if (grid < 1) return LP_OK;
-    cudaError_t le = launch_pdl(gemm_tc_kernel<MODE>, dim3(grid), dim3(GEMM_THREADS), GEMM_SMEM, stream, a0, a1, b, p);
+    cudaError_t le = launch_pdl(gemm_tc_kernel<MODE, ACT>, dim3(grid), dim3(GEMM_THREADS), GEMM_SMEM, stream, a0, a1, b, p);
     if (le != cudaSuccess) return cuda_fail(le, "launch gemm_tc_kernel");
     LP_LAUNCH_CHECK("gemm_tc_kernel");
     return LP_OK;
@@ -252,7 +253,7 @@ bool deconv_rows_shape_ok(int W);
 size_t deconv_rows_packed_elems(int Cr, int Cw, int Co);
 void deconv_rows_pack(const uint16_t* wr, const uint16_t* ww, int Cr, int Cw, int Co, uint16_t* wp);
 int launch_deconv_rows(const void* refined, const void* raw, const void* w_rows, const float* bias_packed, void* out, int N,
-                       int H, int W, int Cr, int Cw, int Co, cudaStream_t stream);
+                       int H, int W, int Cr, int Cw, int Co, int act, cudaStream_t stream);
 }  // namespace lp
 
 static int deconv_ntile(int Co) { return round_up(Co, 16); }
@@ -329,9 +330,11 @@ extern "C" int lp_deconv_pack(const uint16_t* wr, const uint16_t* ww, const floa
     return LP_OK;
 }
 
-extern "C" int lp_fusion_deconv_f16(const void* refined, const void* raw, const void* w_packed, const float* bias_packed,
-                                    void* out, int N, int H, int W, int Cr, int Cw, int Co, lp_stream_t stream) {
+extern "C" int lp_fusion_deconv_act_f16(const void* refined, const void* raw, const void* w_packed,
+                                        const float* bias_packed, void* out, int N, int H, int W, int Cr, int Cw, int Co,
+                                        int act, lp_stream_t stream) {
     LP_CHECK_ARG(refined && (raw || Cw == 0) && w_packed && out, "lp_fusion_deconv_f16: null pointer");
+    LP_CHECK_ARG(act == LP_ACT_RELU || act == LP_ACT_NONE, "lp_fusion_deconv_act_f16: act %d (ReLU or none)", act);
     LP_CHECK_ARG(N > 0 && H > 0 && W > 0 && Cr % 8 == 0 && Cw % 8 == 0 && Co % 8 == 0 && Co >= 8 && Co <= 64,
                  "lp_fusion_deconv_f16: bad shape N=%d H=%d W=%d Cr=%d Cw=%d Co=%d (Co<=64)", N, H, W, Cr, Cw, Co);
     GemmParams p;
@@ -347,7 +350,7 @@ extern "C" int lp_fusion_deconv_f16(const void* refined, const void* raw, const 
     }
     if (deconv_rows_channels_ok(Cr, Cw, Co) && deconv_rows_shape_ok(W)) {
         const uint16_t* w_rows = reinterpret_cast<const uint16_t*>(w_packed) + (size_t)p.total_bt * p.n_tile * BK;
-        return launch_deconv_rows(refined, raw, w_rows, bias_packed, out, N, H, W, Cr, Cw, Co, (cudaStream_t)stream);
+        return launch_deconv_rows(refined, raw, w_rows, bias_packed, out, N, H, W, Cr, Cw, Co, act, (cudaStream_t)stream);
     }
     pick_spatial_tile(H, W, &p.TH, &p.TW);
     p.tiles_x = (W + p.TW - 1) / p.TW;
@@ -356,7 +359,7 @@ extern "C" int lp_fusion_deconv_f16(const void* refined, const void* raw, const 
     p.H = H;
     p.W = W;
     p.N = Co;
-    p.act = LP_ACT_RELU;
+    p.act = act;
     p.bias = bias_packed;
     p.out = out;
     CUtensorMap m0, m1, mb;
@@ -370,7 +373,13 @@ extern "C" int lp_fusion_deconv_f16(const void* refined, const void* raw, const 
     }
     rc = make_tmap_rows64(&mb, w_packed, p.total_bt * p.n_tile, BK, p.n_tile, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
-    return launch_gemm<MODE_DECONV>(m0, m1, mb, p, (cudaStream_t)stream);
+    if (act == LP_ACT_RELU) return launch_gemm<MODE_DECONV, LP_ACT_RELU>(m0, m1, mb, p, (cudaStream_t)stream);
+    return launch_gemm<MODE_DECONV, LP_ACT_NONE>(m0, m1, mb, p, (cudaStream_t)stream);
+}
+
+extern "C" int lp_fusion_deconv_f16(const void* refined, const void* raw, const void* w_packed, const float* bias_packed,
+                                    void* out, int N, int H, int W, int Cr, int Cw, int Co, lp_stream_t stream) {
+    return lp_fusion_deconv_act_f16(refined, raw, w_packed, bias_packed, out, N, H, W, Cr, Cw, Co, LP_ACT_RELU, stream);
 }
 
 // ------------------------------------------------------------------ heads

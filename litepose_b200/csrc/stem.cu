@@ -1,4 +1,5 @@
-// Stem: conv3x3 stride 2 (3 -> 32) + folded-BN bias + ReLU6; reads the reference's NCHW input
+// Stem: conv3x3 stride 2 (3 -> 32) + folded-BN bias + ReLU6 (or no activation: the raw convolution the BN
+// recalibration pass takes its batch statistics of, lp_stem_conv3x3_s2_act); reads the reference's NCHW input
 // (fp32, or fp16 under network_to_half) and writes the NHWC fp16 activation layout used by all
 // later kernels.  Reference: convbnrelu(3, 32, ker=3, stride=2), lib/models/pose_mobilenet.py:37,
 // lib/models/layers/layers.py:18-24.
@@ -21,7 +22,12 @@ template <typename TIn> struct StemVec;
 template <> struct StemVec<__half> { static constexpr int N = 8; };   // 16-byte global vectors
 template <> struct StemVec<float> { static constexpr int N = 4; };
 
-template <typename TIn, bool VEC>
+template <int ACT>
+__device__ __forceinline__ float stem_act(float v) {
+    return ACT == LP_ACT_RELU6 ? fminf(fmaxf(v, 0.f), 6.f) : v;
+}
+
+template <typename TIn, bool VEC, int ACT>
 __global__ void __launch_bounds__(256)
 stem_kernel(const TIn* __restrict__ x, const __half* __restrict__ w, const float* __restrict__ bias,
             __half* __restrict__ y, int H, int W, int flip_x) {
@@ -177,8 +183,7 @@ stem_kernel(const TIn* __restrict__ x, const __half* __restrict__ w, const float
                 __half2* h = reinterpret_cast<__half2*>(&o);
 #pragma unroll
                 for (int i = 0; i < 4; ++i)
-                    h[i] = __floats2half2_rn(fminf(fmaxf(acc[8 * g + 2 * i], 0.f), 6.f),
-                                             fminf(fmaxf(acc[8 * g + 2 * i + 1], 0.f), 6.f));
+                    h[i] = __floats2half2_rn(stem_act<ACT>(acc[8 * g + 2 * i]), stem_act<ACT>(acc[8 * g + 2 * i + 1]));
                 op[g] = o;
             }
         }
@@ -189,29 +194,42 @@ stem_kernel(const TIn* __restrict__ x, const __half* __restrict__ w, const float
 
 using namespace lp;
 
-extern "C" int lp_stem_conv3x3_s2(const void* x, int x_is_fp32, int flip_x, const void* w, const float* bias, void* y,
-                                  int N, int H, int W, lp_stream_t stream) {
+template <int ACT>
+static void stem_launch(const void* x, int x_is_fp32, int flip_x, const __half* wh, const float* bias, __half* yh, int N,
+                        int H, int W, cudaStream_t st) {
+    dim3 grid((W / 2 + ST_TW - 1) / ST_TW, (H / 2 + ST_TH - 1) / ST_TH, N);
+    const bool aligned = (reinterpret_cast<uintptr_t>(x) & 15) == 0;
+    if (x_is_fp32) {
+        const float* xf = reinterpret_cast<const float*>(x);
+        if (aligned && W % 4 == 0) stem_kernel<float, true, ACT><<<grid, 256, 0, st>>>(xf, wh, bias, yh, H, W, flip_x);
+        else stem_kernel<float, false, ACT><<<grid, 256, 0, st>>>(xf, wh, bias, yh, H, W, flip_x);
+    } else {
+        const __half* xh = reinterpret_cast<const __half*>(x);
+        if (aligned && W % 8 == 0) stem_kernel<__half, true, ACT><<<grid, 256, 0, st>>>(xh, wh, bias, yh, H, W, flip_x);
+        else stem_kernel<__half, false, ACT><<<grid, 256, 0, st>>>(xh, wh, bias, yh, H, W, flip_x);
+    }
+}
+
+extern "C" int lp_stem_conv3x3_s2_act(const void* x, int x_is_fp32, int flip_x, const void* w, const float* bias,
+                                      void* y, int N, int H, int W, int act, lp_stream_t stream) {
     LP_CHECK_ARG(x && w && y, "lp_stem_conv3x3_s2: null pointer");
     LP_CHECK_ARG(N > 0 && N <= 65535 && H > 0 && W > 0 && H % 2 == 0 && W % 2 == 0,
                  "lp_stem_conv3x3_s2: bad shape N=%d H=%d W=%d (H, W even)", N, H, W);
+    LP_CHECK_ARG(act == LP_ACT_RELU6 || act == LP_ACT_NONE, "lp_stem_conv3x3_s2_act: act %d (ReLU6 or none)", act);
     if (reinterpret_cast<uintptr_t>(y) & 15) {
         set_error("lp_stem_conv3x3_s2: y must be 16-byte aligned");
         return LP_ERR_ALIGN;
     }
-    dim3 grid((W / 2 + ST_TW - 1) / ST_TW, (H / 2 + ST_TH - 1) / ST_TH, N);
-    const bool aligned = (reinterpret_cast<uintptr_t>(x) & 15) == 0;
     const __half* wh = reinterpret_cast<const __half*>(w);
     __half* yh = reinterpret_cast<__half*>(y);
     cudaStream_t st = (cudaStream_t)stream;
-    if (x_is_fp32) {
-        const float* xf = reinterpret_cast<const float*>(x);
-        if (aligned && W % 4 == 0) stem_kernel<float, true><<<grid, 256, 0, st>>>(xf, wh, bias, yh, H, W, flip_x);
-        else stem_kernel<float, false><<<grid, 256, 0, st>>>(xf, wh, bias, yh, H, W, flip_x);
-    } else {
-        const __half* xh = reinterpret_cast<const __half*>(x);
-        if (aligned && W % 8 == 0) stem_kernel<__half, true><<<grid, 256, 0, st>>>(xh, wh, bias, yh, H, W, flip_x);
-        else stem_kernel<__half, false><<<grid, 256, 0, st>>>(xh, wh, bias, yh, H, W, flip_x);
-    }
+    if (act == LP_ACT_RELU6) stem_launch<LP_ACT_RELU6>(x, x_is_fp32, flip_x, wh, bias, yh, N, H, W, st);
+    else stem_launch<LP_ACT_NONE>(x, x_is_fp32, flip_x, wh, bias, yh, N, H, W, st);
     LP_LAUNCH_CHECK("stem_kernel");
     return LP_OK;
+}
+
+extern "C" int lp_stem_conv3x3_s2(const void* x, int x_is_fp32, int flip_x, const void* w, const float* bias, void* y,
+                                  int N, int H, int W, lp_stream_t stream) {
+    return lp_stem_conv3x3_s2_act(x, x_is_fp32, flip_x, w, bias, y, N, H, W, LP_ACT_RELU6, stream);
 }

@@ -11,8 +11,11 @@ shapes and creation order equal the reference's (pose_supermobilenet.py:23-63, l
 ``search_arch`` when ``is_search`` is set).  In eval mode on a CUDA tensor it then runs that sub-network on the sm_90a
 kernels: ``litepose_b200.subnet.derive_supernet_subnet`` applies the supernet's rules (prefix slices, the k = 5 / 3
 depthwise transform, its own strides and identity adds) and a ``LitePoseEngine`` runs the result; engines are cached
-per (device, architecture), a few at a time.  CPU tensors and training mode (the BN recalibration pass of the search)
-run the module tree.
+per (device, architecture), a few at a time.  CPU tensors and training mode run the module tree.
+
+``lp_recalibrate_bn(x)`` is the search's BN recalibration pass (calibrate_test.py: ``model.train(); model(images)``) on
+the kernels: it does to the module's BatchNorm buffers what a train-mode forward does, without autograd, and returns
+what that forward returns (litepose_b200.bn_train).
 
 One deviation: the reference's ``SuperConvTranspose2d.forward`` calls ``_output_padding`` with the argument list of
 torch 1.x, which raises ``TypeError`` on torch >= 2.0 (the method gained ``num_spatial_dims``), so the reference module
@@ -32,6 +35,8 @@ from .pose_mobilenet import convbnrelu
 
 # engines kept per module: a search evaluates one candidate after another, a training run draws a new one per step
 ENGINE_LRU = 4
+# train-mode plans kept per module (BN recalibration): one per (device, architecture, input shape)
+TRAIN_PLAN_LRU = 4
 
 
 class SuperBatchNorm2d(nn.BatchNorm2d):
@@ -172,6 +177,7 @@ class SuperLitePose(EngineModule):
         self.num_deconv_layers = extra.NUM_DECONV_LAYERS
         self.loss_config = cfg.LOSS
         self._lp_cache = _EngineCache()
+        self._lp_train_cache = _EngineCache()
 
     # -- engine ----------------------------------------------------------------
     def lp_engine(self, device=None, cfg_arch=None):
@@ -200,6 +206,84 @@ class SuperLitePose(EngineModule):
             # CUDA inference: hand-written sm_90a kernels only (raises if the library is missing)
             return self.lp_engine(x.device, cfg_arch).run(x, flip=False, out_fp32=x.dtype != torch.float16, clone=True)
         return self._forward_modules(x, cfg_arch)
+
+    # -- BN recalibration -------------------------------------------------------
+    def lp_recalibrate_bn(self, x):
+        """What ``model.train(); model(x)`` does to this module, on the sm_90a kernels, without autograd: one
+        ``arch_manager.random_sample()`` (as ``forward``), then the sub-network's train-mode forward.  Every BatchNorm
+        it runs takes the batch statistics (biased variance) for the normalisation and updates its running statistics
+        to (1 - momentum) * running + momentum * batch statistic (unbiased variance), the leading [:c] slice of a
+        SuperBatchNorm2d only; num_batches_tracked grows by one on the plain BatchNorm2d of first.0 / first.1 (the
+        SuperBatchNorm2d call F.batch_norm, which does not count).  The train / eval mode is left as it is.
+
+        x: NCHW CUDA tensor, fp32 (fp16 under network_to_half).  Returns the outputs of the train-mode forward (fp32,
+        fp16 for an fp16 x; they do not require grad).  The new statistics are staged on the device and copied into the
+        buffers only once all of them are finite: otherwise ``LitePoseError`` names the layers and no buffer changes.
+        Raises ValueError for a CPU tensor, a BatchNorm with momentum None, one value per channel (N*H*W == 1) and
+        shapes the kernels do not take."""
+        from litepose_b200 import bn_train
+        from litepose_b200._lib import LitePoseError
+        cfg_arch = self.arch_manager.random_sample()
+        if not torch.is_tensor(x) or x.dim() != 4 or x.shape[1] != 3 or x.dtype not in (torch.float16, torch.float32):
+            raise ValueError("lp_recalibrate_bn takes an NCHW 3-channel fp32 or fp16 image batch, got %s"
+                             % ((tuple(x.shape), x.dtype) if torch.is_tensor(x) else type(x).__name__,))
+        names = bn_train.bn_names(cfg_arch)
+        mods = [self.get_submodule(n) for n in names]
+        for n, m in zip(names, mods):
+            if m.momentum is None:
+                raise ValueError("%s: momentum None (a cumulative average) is not supported; the supernet's "
+                                 "F.batch_norm call cannot take it either" % n)
+            if not m.track_running_stats:
+                raise ValueError("%s keeps no running statistics to recalibrate" % n)
+        n_, _, h, w = x.shape
+        if h % 16 or w % 16:
+            raise ValueError("LitePose input height/width must be multiples of 16, got %dx%d" % (h, w))
+        if n_ * (h // 16) * (w // 16) <= 1:
+            raise ValueError("input %s leaves one value per channel at the backbone's last stage; train-mode BatchNorm "
+                             "needs more than one (N*H*W > 1)" % (tuple(x.shape),))
+        if not x.is_cuda:
+            raise ValueError("lp_recalibrate_bn runs on the GPU kernels: it needs a CUDA tensor (the module tree runs "
+                             "CPU tensors: model.train(); model(x))")
+        plan = self._lp_train_plan(x, cfg_arch, names, mods)
+        running = [(m.running_mean[:c], m.running_var[:c]) for m, c in zip(mods, plan.channels)]
+        outs, staged = plan.run(x, running)
+        flags = plan.flags.cpu()
+        if bool(flags.any()):
+            bad = [n for n, f in zip(names, flags.tolist()) if f]
+            raise LitePoseError("BN recalibration: non-finite batch statistics in %s (no buffer was changed)"
+                                % ", ".join(bad))
+        dst, src = [], []
+        for i, (m, c) in enumerate(zip(mods, plan.channels)):
+            o = int(plan.offs[i])
+            dst += [m.running_mean[:c], m.running_var[:c]]
+            src += [staged[2, o:o + c], staged[3, o:o + c]]
+        with torch.no_grad():
+            torch._foreach_copy_(dst, src)      # in place: the version counters move, so the eval engine repacks
+            for m in mods:
+                if not isinstance(m, SuperBatchNorm2d) and m.num_batches_tracked is not None:
+                    m.num_batches_tracked.add_(1)
+        return outs
+
+    def _lp_train_plan(self, x, cfg_arch, names, mods):
+        """The cached train-mode plan of ``cfg_arch`` at x's shape, rebuilt when a parameter or a BatchNorm's
+        momentum / eps changed (the running statistics are read at every run)"""
+        from litepose_b200 import bn_train
+        from litepose_b200.subnet import derive_supernet_subnet
+        key = self._lp_device_key(x.device) + (_arch_key(cfg_arch), tuple(x.shape), x.dtype)
+        sig = hash(tuple((id(t), t.data_ptr(), t._version) for t in self.parameters()) +
+                   tuple((m.momentum, m.eps) for m in mods))
+        cache = self._lp_train_cache
+        with cache.lock:
+            hit = cache.engines.pop(key, None)
+            if hit is None or hit[1] != sig:
+                sub = derive_supernet_subnet(self.state_dict(), cfg_arch)
+                params = {n: (m.momentum, m.eps) for n, m in zip(names, mods)}
+                n, _, h, w = x.shape
+                hit = (bn_train.BNTrainPlan(sub, params, x.device, n, h, w, x.dtype), sig)
+            cache.engines[key] = hit
+            while len(cache.engines) > TRAIN_PLAN_LRU:
+                del cache.engines[next(iter(cache.engines))]
+            return hit[0]
 
     def _forward_modules(self, x, cfg_arch):
         x = self.first[1](self.first[0](x))
