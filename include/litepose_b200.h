@@ -214,6 +214,13 @@ int lp_head_fused_f16(const void* a1, const void* a2, const void* dw_cat, const 
                       const void* pw_packed, void* out_nchw, int out_fp32, int N, int H, int W, int C1,
                       int C2, int Co, lp_stream_t stream);
 
+/* Largest K (= MAX_NUM_PEOPLE) the evaluation parser takes: top-K slots per (image, joint) plane and the side of
+ * the matcher's cost matrices.  K <= 64 runs on per-warp lists and one warp per image; 64 < K <= 256 on per-CTA
+ * candidate buffers and one CTA per image with its cost matrices in the caller's workspace.  The uniform entry
+ * points lp_nms_topk_f32 / lp_tag_match_f32 keep K <= 64; K up to LP_PARSER_MAX_PEOPLE goes through the ragged
+ * entry points (a uniform batch is N equal lp_map_desc_t entries, with the same results per image). */
+#define LP_PARSER_MAX_PEOPLE 256
+
 /* ---- G1+G2: NMS (k x k window max, -inf padding) + top-K per (n,j) plane -----
  * det fp32 [N,J,H,W]; tag fp32 [N,J,H,W,T].  Order: value desc, flat index asc over
  * NMS survivors with value > 0; unused slots are (0.0f, index 0).  NaN never takes a slot, and
@@ -221,7 +228,8 @@ int lp_head_fused_f16(const void* a1, const void* a2, const void* dw_cat, const 
  * nms_kernel odd, 1..9.  Width bound (one fp32 strip buffer of at most 200 KB in shared memory):
  * W <= 51200 / (nms_kernel + 1), e.g. 8533 at kernel 5; wider maps return LP_ERR_BAD_ARG.
  * Any height is accepted.
- * val_k [N,J,K] f32; ind_k [N,J,K] i32 (flat y*W+x); tag_k [N,J,K,T] f32.  K <= 64.
+ * val_k [N,J,K] f32; ind_k [N,J,K] i32 (flat y*W+x); tag_k [N,J,K,T] f32.  K <= 64
+ * (lp_nms_topk_ragged_f32: K <= LP_PARSER_MAX_PEOPLE).
  * min_value (double, compared as the reference does: float32 value widened to double): only survivors
  * with value > max(min_value, 0) are reported.  0 reproduces top_k as the
  * reference computes it; the full parse passes DETECTION_THRESHOLD, because match_by_tag drops every
@@ -238,7 +246,9 @@ int lp_nms_topk_f32(const float* det, const float* tag, int N, int J, int H, int
  * LP_ERR_CAPACITY is NOT raised on the device; the caller compares against pcap;
  * pcap = J*K can never overflow).  Thresholds are doubles because the reference
  * compares float64 joint rows against Python floats (group.py:38-41,84).
- * K, max_num_people <= 64 (one cost-matrix column per lane up to 32, two above). */
+ * K <= 64 (lp_tag_match_ragged_f32: K <= LP_PARSER_MAX_PEOPLE).  K <= 64: max_num_people <= 64, one warp
+ * per image (one cost-matrix column per lane up to 32, two above).  K > 64 (ragged entry): max_num_people <= K, one 256-thread CTA per image; its two fp64
+ * K x K matrices (costs, distances) live in the workspace, which lp_tag_match_workspace_bytes sizes from K. */
 size_t lp_tag_match_workspace_bytes(int N, int J, int K, int T, int pcap);
 int lp_tag_match_f32(const float* val_k, const int32_t* ind_k, const float* tag_k, int N, int J,
                      int K, int T, int W, const int32_t* joint_order, double det_threshold,

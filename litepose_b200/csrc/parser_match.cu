@@ -2,9 +2,10 @@
 // (reference lib/core/group.py:19-97; third-party `munkres` package restated in
 // oracle/munkres_ref.py, SURVEY.md Appendix A.7/A.8).
 //
-// One warp per image (images are independent, SURVEY H5); joints are processed sequentially in
-// joint_order like the reference, the inner searches/reductions run across the 32 lanes
-// (lane <-> cost-matrix column).  Bit-exact requirements reproduced here:
+// One warp per image for K <= 64, one CTA per image above (images are independent, SURVEY H5); joints are processed
+// sequentially in joint_order like the reference, the inner searches/reductions run across the threads
+// (thread <-> cost-matrix column).  The per-joint logic is one template (match_image) over the three Munkres cores.
+// Bit-exact requirements reproduced here:
 //   * joints rows are float64 in the reference: the threshold tests run in double;
 //   * running person tag = np.mean(list of f32 vectors, axis=0): sequential f32 sum / count for
 //     T >= 2, numpy's 8-accumulator pairwise sum for T == 1 (measured, see oracle/group_ref.py);
@@ -166,154 +167,8 @@ struct MatchArgs {
     int use_det_val, ignore_too_much, max_people, pcap;
     float* ans; int32_t* num_people;
     float* pkey; int32_t* ptagn; float* ptags;   // workspace
+    double* mat;                                 // workspace, K > 64: per image the K x K cost and distance matrices
 };
-
-__device__ int find_person(const MatchArgs& a, const float* pkey, int P, float key, int lane) {
-    const int lim = P < a.pcap ? P : a.pcap;
-    for (int p0 = 0; p0 < lim; p0 += 32) {
-        const int p = p0 + lane;
-        const unsigned m = __ballot_sync(0xffffffffu, p < lim && pkey[p] == key);
-        if (m) return p0 + __ffs(m) - 1;
-    }
-    return -1;
-}
-
-__global__ void __launch_bounds__(32)
-tag_match_kernel(const MatchArgs a) {
-    __shared__ MatchSmem S;
-    const int n = blockIdx.x;
-    const int lane = threadIdx.x;
-    const int J = a.J, K = a.K, T = a.T, D = 3 + a.T;
-    const int W = a.desc ? a.desc[n].w : a.W;
-    float* ans = a.ans + (size_t)n * a.pcap * J * D;
-    float* pkey = a.pkey + (size_t)n * a.pcap;
-    int32_t* ptagn = a.ptagn + (size_t)n * a.pcap;
-    float* ptags = a.ptags + (size_t)n * a.pcap * J * T;
-    int P = 0;
-
-    // setdefault(key, zeros)[idx] = joint ; tag_dict[key] = [tag]
-    auto new_or_reset = [&](int r, int idx) {
-        const float key = S.ct[r][0];
-        int p = find_person(a, pkey, P, key, lane);
-        if (p < 0) {
-            p = P++;
-            if (p < a.pcap) {
-                for (int e = lane; e < J * D; e += 32) ans[(size_t)p * J * D + e] = 0.f;
-                if (lane == 0) pkey[p] = key;
-            }
-        }
-        __syncwarp();
-        if (p < a.pcap) {
-            float* row = ans + ((size_t)p * J + idx) * D;
-            if (lane == 0) {
-                row[0] = (float)S.cx[r];
-                row[1] = (float)S.cy[r];
-                row[2] = S.cv[r];
-                ptagn[p] = 1;
-            }
-            if (lane < T) {
-                row[3 + lane] = S.ct[r][lane];
-                ptags[((size_t)p * J + 0) * T + lane] = S.ct[r][lane];
-            }
-        }
-        __syncwarp();
-    };
-
-    for (int ji = 0; ji < J; ++ji) {
-        const int idx = a.joint_order[ji];
-        const size_t base = ((size_t)n * J + idx) * K;
-        float v = 0.f;
-        bool ok = false;
-        if (lane < K) {
-            v = a.val_k[base + lane];
-            ok = (double)v > a.det_thr;
-        }
-        const unsigned mask = __ballot_sync(0xffffffffu, ok);
-        const int rows = __popc(mask);
-        if (rows == 0) continue;
-        if (ok) {
-            const int r = __popc(mask & ((1u << lane) - 1u));
-            const int ind = a.ind_k[base + lane];
-            S.cx[r] = ind % W;
-            S.cy[r] = ind / W;
-            S.cv[r] = v;
-            for (int t = 0; t < T; ++t) S.ct[r][t] = a.tag_k[(base + lane) * T + t];
-        }
-        __syncwarp();
-
-        if (ji == 0 || P == 0) {
-            for (int r = 0; r < rows; ++r) new_or_reset(r, idx);
-            continue;
-        }
-        const int G = P < a.max_people ? P : a.max_people;
-        if (a.ignore_too_much && G == a.max_people) continue;
-        // running mean tag of each grouped person
-        if (lane < G) {
-            const int cnt = ptagn[lane];
-            const float* tl = ptags + (size_t)lane * J * T;
-            for (int t = 0; t < T; ++t) {
-                float s;
-                if (T == 1) {
-                    s = np_pairwise_sum_f32(tl, cnt, 1);
-                } else {
-                    s = tl[t];
-                    for (int q = 1; q < cnt; ++q) s = __fadd_rn(s, tl[q * T + t]);
-                }
-                S.mean[lane][t] = __fdiv_rn(s, (float)cnt);
-            }
-        }
-        __syncwarp();
-        const int nn = rows > G ? rows : G;
-        for (int r = 0; r < nn; ++r) {
-            if (lane < nn) {
-                double c;
-                if (r >= rows) {
-                    c = 0.0;                       // Munkres pads missing rows with 0
-                } else if (lane < G) {
-                    double d2 = 0.0;
-                    for (int t = 0; t < T; ++t) {
-                        const double dd = __dsub_rn((double)S.ct[r][t], (double)S.mean[lane][t]);
-                        const double sq = __dmul_rn(dd, dd);
-                        d2 = (t == 0) ? sq : __dadd_rn(d2, sq);
-                    }
-                    const double d = sqrt(d2);
-                    S.saved[r][lane] = d;
-                    c = a.use_det_val ? __dsub_rn(__dmul_rn(rint(d), 100.0), (double)S.cv[r]) : d;
-                } else {
-                    c = 1e10;                      // reference pads columns with 1e10 when rows > cols
-                }
-                S.C[r][lane] = c;
-            }
-        }
-        __syncwarp();
-        munkres_warp(S, nn, lane);
-        __syncwarp();
-        for (int r = 0; r < rows; ++r) {
-            const int c = S.star_col[r];
-            const bool accept = (c >= 0) && (c < G) && (S.saved[r][c] < a.tag_thr);
-            if (accept) {
-                const int cnt = ptagn[c];
-                float* row = ans + ((size_t)c * J + idx) * D;
-                __syncwarp();
-                if (lane == 0) {
-                    row[0] = (float)S.cx[r];
-                    row[1] = (float)S.cy[r];
-                    row[2] = S.cv[r];
-                    ptagn[c] = cnt + 1;
-                }
-                if (lane < T) {
-                    row[3 + lane] = S.ct[r][lane];
-                    if (cnt < J) ptags[((size_t)c * J + cnt) * T + lane] = S.ct[r][lane];
-                }
-                __syncwarp();
-            } else {
-                new_or_reset(r, idx);
-            }
-        }
-    }
-    if (lane == 0) a.num_people[n] = P;
-}
-
 
 // ---- wide variant: 32 < MAX_NUM_PEOPLE <= 64 (the reference has no limit, lib/config/default.py MAX_NUM_PEOPLE) ------
 // Same algorithm, same scan orders and the same IEEE operations as above; lane l owns the cost-matrix columns l and
@@ -451,12 +306,261 @@ __device__ void munkres_warp_wide(MatchSmemW& S, const int n, const int lane) {
     }
 }
 
-__global__ void __launch_bounds__(32)
-tag_match_wide_kernel(const MatchArgs a) {
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    MatchSmemW& S = *reinterpret_cast<MatchSmemW*>(smem_raw);
+// ---- one CTA per image: 64 < K <= LP_PARSER_MAX_PEOPLE -------------------------------------------------------------------
+// The same step sequence with thread c <-> cost-matrix column c.  The cost and distance matrices (fp64, K x K each) are in
+// the caller's workspace; shared memory keeps the zero pattern of C as a bitmap (rebuilt by step 1 and every step 6, the
+// only steps that change C), so the step-4 scans test 32 columns per word.  Step 4 looks at all uncovered rows at once
+// (thread t takes the t-th row of the cyclic order), step 6 is one pass over C per column thread.
+constexpr int MC = LP_PARSER_MAX_PEOPLE;     // max matrix side
+constexpr int MC_THREADS = MC;               // one thread per column
+constexpr int MC_WARPS = MC_THREADS / 32;
+constexpr int MC_WORDS = MC / 32;            // 32-column words of a bitmap row
+
+struct MatchSmemC {
+    float ct[MC][8];
+    float mean[MC][8];
+    float cv[MC];
+    int cx[MC], cy[MC];
+    int star_col[MC], star_row[MC], prime_col[MC];
+    unsigned zero[MC][MC_WORDS];             // bit c of row i: C[i][c] == 0
+    unsigned row_cov[MC_WORDS], col_cov[MC_WORDS];
+    int red[MC_WARPS];                       // per-warp partial results of block reductions
+    double dred[MC_WARPS];
+};
+
+__device__ __forceinline__ bool bitw(const unsigned* m, int i) { return (m[i >> 5] >> (i & 31)) & 1u; }
+
+// highest uncovered zero of row i below column lim, -1 if none
+__device__ __forceinline__ int highest_below(const MatchSmemC& S, int i, int lim) {
+    for (int q = (lim - 1) >> 5; q >= 0; --q) {
+        unsigned w = S.zero[i][q] & ~S.col_cov[q];
+        if (q == ((lim - 1) >> 5) && (lim & 31)) w &= (1u << (lim & 31)) - 1u;
+        if (w) return 32 * q + 31 - __clz(w);
+    }
+    return -1;
+}
+
+// rows i of C: zero bitmap words from the lanes' values (warp w of the CTA holds columns 32w..32w+31)
+__device__ __forceinline__ void zero_word(MatchSmemC& S, int i, bool z) {
+    const unsigned b = __ballot_sync(0xffffffffu, z);
+    if ((threadIdx.x & 31) == 0) S.zero[i][threadIdx.x >> 5] = b;
+}
+
+// Munkres on the n x n matrix C (row stride ld, n <= MC); result in S.star_col[row]
+__device__ void munkres_cta(MatchSmemC& S, double* C, int ld, const int n) {
+    const double INF = __longlong_as_double(0x7ff0000000000000ll);
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const bool act = tid < n;
+    // step 1: one warp per row
+    for (int i = warp; i < n; i += MC_WARPS) {
+        double m = INF;
+        for (int c = lane; c < n; c += 32) { const double v = C[(size_t)i * ld + c]; m = v < m ? v : m; }
+        m = warp_min_d(m);
+        for (int c = lane; c < n; c += 32) C[(size_t)i * ld + c] = C[(size_t)i * ld + c] - m;
+    }
+    S.star_col[tid] = -1; S.star_row[tid] = -1; S.prime_col[tid] = -1;
+    __syncthreads();
+    for (int i = 0; i < n; ++i) zero_word(S, i, act && C[(size_t)i * ld + tid] == 0.0);
+    __syncthreads();
+    // step 2: greedy starring, row-major, by warp 0 (lane q < MC_WORDS holds cover word q)
+    if (warp == 0) {
+        unsigned cov = 0;
+        for (int i = 0; i < n; ++i) {
+            const unsigned z = lane < MC_WORDS ? S.zero[i][lane] & ~cov : 0u;
+            const unsigned b = __ballot_sync(0xffffffffu, z != 0u);
+            if (b) {
+                const int q = __ffs(b) - 1;
+                const unsigned zq = __shfl_sync(0xffffffffu, z, q);
+                const int j = 32 * q + __ffs(zq) - 1;
+                if (lane == 0) { S.star_col[i] = j; S.star_row[j] = i; }
+                if (lane == q) cov |= 1u << (j & 31);
+            }
+        }
+    }
+    __syncthreads();
+    for (;;) {
+        // step 3
+        const unsigned starred = __ballot_sync(0xffffffffu, act && S.star_row[tid] >= 0);
+        if (lane == 0) { S.col_cov[warp] = starred; S.row_cov[warp] = 0u; }
+        if (__syncthreads_count(act && S.star_row[tid] >= 0) >= n) break;
+        // step 4 (+ step 6 when no uncovered zero is left)
+        int row = 0, col = 0;
+        int z0r = -1, z0c = -1;
+        for (;;) {
+            // the first uncovered row, in cyclic order from `row`, with an uncovered zero
+            bool has = false;
+            if (act) {
+                int i = row + tid;
+                if (i >= n) i -= n;
+                if (!bitw(S.row_cov, i))
+                    for (int q = 0; q < MC_WORDS; ++q) has |= (S.zero[i][q] & ~S.col_cov[q]) != 0u;
+            }
+            const unsigned hb = __ballot_sync(0xffffffffu, has);
+            if (lane == 0) S.red[warp] = hb ? 32 * warp + __ffs(hb) - 1 : MC;
+            __syncthreads();
+            int t = MC;
+#pragma unroll
+            for (int w = 0; w < MC_WARPS; ++w) t = S.red[w] < t ? S.red[w] : t;
+            if (t == MC) {
+                // step 6
+                double m = INF;
+                const bool cu = act && !bitw(S.col_cov, tid);
+                if (cu)
+                    for (int i = 0; i < n; ++i)
+                        if (!bitw(S.row_cov, i)) { const double v = C[(size_t)i * ld + tid]; m = v < m ? v : m; }
+                m = warp_min_d(m);
+                if (lane == 0) S.dred[warp] = m;
+                __syncthreads();
+                m = INF;
+#pragma unroll
+                for (int w = 0; w < MC_WARPS; ++w) m = S.dred[w] < m ? S.dred[w] : m;
+                for (int i = 0; i < n; ++i) {
+                    bool z = false;
+                    if (act) {
+                        double v = C[(size_t)i * ld + tid];
+                        if (bitw(S.row_cov, i)) v = __dadd_rn(v, m);
+                        if (cu) v = __dsub_rn(v, m);
+                        C[(size_t)i * ld + tid] = v;
+                        z = v == 0.0;
+                    }
+                    zero_word(S, i, z);
+                }
+                __syncthreads();
+                row = 0;
+                col = 0;
+                continue;
+            }
+            int fr = row + t;
+            if (fr >= n) fr -= n;
+            int fc = highest_below(S, fr, col);              // columns scanned after the wrap-around
+            if (fc < 0) fc = highest_below(S, fr, MC);
+            const int sc = S.star_col[fr];
+            __syncthreads();                                 // every thread has read the covers and S.red
+            if (sc >= 0) {
+                if (tid == 0) {
+                    S.prime_col[fr] = fc;
+                    S.row_cov[fr >> 5] |= 1u << (fr & 31);
+                    S.col_cov[sc >> 5] &= ~(1u << (sc & 31));
+                }
+                __syncthreads();
+                row = fr;
+                col = sc;
+            } else {
+                if (tid == 0) S.prime_col[fr] = fc;
+                z0r = fr;
+                z0c = fc;
+                break;
+            }
+        }
+        // step 5
+        __syncthreads();
+        if (tid == 0) {
+            int r = z0r, c = z0c;
+            for (;;) {
+                const int sr = S.star_row[c];
+                S.star_row[c] = r;
+                S.star_col[r] = c;
+                if (sr < 0) break;
+                r = sr;
+                c = S.prime_col[sr];
+            }
+        }
+        __syncthreads();
+        S.prime_col[tid] = -1;
+        __syncthreads();
+    }
+}
+
+// ---- match_by_tag, shared by the three matchers -------------------------------------------------------------------------
+// A matcher M brings its thread count NT, its storage (M::C/saved/ct/mean/cv/cx/cy/star_col) and its Munkres core;
+// the per-joint logic below (thresholds in double, running means, dict-keyed persons, IGNORE_TOO_MUCH, the grouped
+// prefix of max_num_people) is written once for all of them.
+__device__ __forceinline__ void munkres_core(MatchSmem& S, int n, int lane) { munkres_warp(S, n, lane); }
+__device__ __forceinline__ void munkres_core(MatchSmemW& S, int n, int lane) { munkres_warp_wide(S, n, lane); }
+
+template <class SM>
+struct WarpMatcher {                          // one warp per image, matrices in shared memory
+    static constexpr int NT = 32;
+    SM& S;
+    __device__ double& C(int r, int c) { return S.C[r][c]; }
+    __device__ double& saved(int r, int c) { return S.saved[r][c]; }
+    __device__ float* ct(int r) { return S.ct[r]; }
+    __device__ float* mean(int g) { return S.mean[g]; }
+    __device__ float& cv(int r) { return S.cv[r]; }
+    __device__ int& cx(int r) { return S.cx[r]; }
+    __device__ int& cy(int r) { return S.cy[r]; }
+    __device__ int star_col(int r) { return S.star_col[r]; }
+    __device__ int* red() { return nullptr; }
+    __device__ static void sync() { __syncwarp(); }
+    __device__ void munkres(int n) { munkres_core(S, n, threadIdx.x); }
+};
+
+struct CtaMatcher {                           // one CTA per image, matrices in the workspace
+    static constexpr int NT = MC_THREADS;
+    MatchSmemC& S;
+    double* Cm;
+    double* Sv;
+    int ld;
+    __device__ double& C(int r, int c) { return Cm[(size_t)r * ld + c]; }
+    __device__ double& saved(int r, int c) { return Sv[(size_t)r * ld + c]; }
+    __device__ float* ct(int r) { return S.ct[r]; }
+    __device__ float* mean(int g) { return S.mean[g]; }
+    __device__ float& cv(int r) { return S.cv[r]; }
+    __device__ int& cx(int r) { return S.cx[r]; }
+    __device__ int& cy(int r) { return S.cy[r]; }
+    __device__ int star_col(int r) { return S.star_col[r]; }
+    __device__ int* red() { return S.red; }
+    __device__ static void sync() { __syncthreads(); }
+    __device__ void munkres(int n) { munkres_cta(S, Cm, ld, n); }
+};
+
+// lowest thread index whose pred holds (-1 if none), the same in every thread
+template <int NT>
+__device__ __forceinline__ int first_thread(bool pred, int* red) {
+    const unsigned m = __ballot_sync(0xffffffffu, pred);
+    if (NT == 32) return m ? __ffs(m) - 1 : -1;
+    const int warp = threadIdx.x >> 5;
+    if ((threadIdx.x & 31) == 0) red[warp] = m ? 32 * warp + __ffs(m) - 1 : NT;
+    __syncthreads();
+    int f = NT;
+    for (int w = 0; w < NT / 32; ++w) f = red[w] < f ? red[w] : f;
+    __syncthreads();
+    return f == NT ? -1 : f;
+}
+
+// number of lower threads whose pred holds; *total = number of threads whose pred holds
+template <int NT>
+__device__ __forceinline__ int thread_rank(bool pred, int* red, int* total) {
+    const unsigned m = __ballot_sync(0xffffffffu, pred);
+    const int lane = threadIdx.x & 31;
+    const int below = __popc(m & ((1u << lane) - 1u));
+    if (NT == 32) { *total = __popc(m); return below; }
+    const int warp = threadIdx.x >> 5;
+    if (lane == 0) red[warp] = __popc(m);
+    __syncthreads();
+    int pre = 0, tot = 0;
+    for (int w = 0; w < NT / 32; ++w) { pre += w < warp ? red[w] : 0; tot += red[w]; }
+    __syncthreads();
+    *total = tot;
+    return pre + below;
+}
+
+template <class M>
+__device__ int find_person(const MatchArgs& a, M& m, const float* pkey, int P, float key) {
+    const int lim = P < a.pcap ? P : a.pcap;
+    for (int p0 = 0; p0 < lim; p0 += M::NT) {
+        const int p = p0 + threadIdx.x;
+        const int f = first_thread<M::NT>(p < lim && pkey[p] == key, m.red());
+        if (f >= 0) return p0 + f;
+    }
+    return -1;
+}
+
+template <class M>
+__device__ void match_image(const MatchArgs& a, M& m) {
+    constexpr int NT = M::NT;
     const int n = blockIdx.x;
-    const int lane = threadIdx.x;
+    const int tid = threadIdx.x;
     const int J = a.J, K = a.K, T = a.T, D = 3 + a.T;
     const int W = a.desc ? a.desc[n].w : a.W;
     float* ans = a.ans + (size_t)n * a.pcap * J * D;
@@ -465,60 +569,60 @@ tag_match_wide_kernel(const MatchArgs a) {
     float* ptags = a.ptags + (size_t)n * a.pcap * J * T;
     int P = 0;
 
+    // setdefault(key, zeros)[idx] = joint ; tag_dict[key] = [tag]
     auto new_or_reset = [&](int r, int idx) {
-        const float key = S.ct[r][0];
-        int p = find_person(a, pkey, P, key, lane);
+        const float key = m.ct(r)[0];
+        int p = find_person(a, m, pkey, P, key);
         if (p < 0) {
             p = P++;
             if (p < a.pcap) {
-                for (int e = lane; e < J * D; e += 32) ans[(size_t)p * J * D + e] = 0.f;
-                if (lane == 0) pkey[p] = key;
+                for (int e = tid; e < J * D; e += NT) ans[(size_t)p * J * D + e] = 0.f;
+                if (tid == 0) pkey[p] = key;
             }
         }
-        __syncwarp();
+        m.sync();
         if (p < a.pcap) {
             float* row = ans + ((size_t)p * J + idx) * D;
-            if (lane == 0) {
-                row[0] = (float)S.cx[r];
-                row[1] = (float)S.cy[r];
-                row[2] = S.cv[r];
+            if (tid == 0) {
+                row[0] = (float)m.cx(r);
+                row[1] = (float)m.cy(r);
+                row[2] = m.cv(r);
                 ptagn[p] = 1;
             }
-            if (lane < T) {
-                row[3 + lane] = S.ct[r][lane];
-                ptags[((size_t)p * J + 0) * T + lane] = S.ct[r][lane];
+            if (tid < T) {
+                row[3 + tid] = m.ct(r)[tid];
+                ptags[((size_t)p * J + 0) * T + tid] = m.ct(r)[tid];
             }
         }
-        __syncwarp();
+        m.sync();
     };
 
     for (int ji = 0; ji < J; ++ji) {
         const int idx = a.joint_order[ji];
         const size_t base = ((size_t)n * J + idx) * K;
-        float v[2] = {0.f, 0.f};
-        bool ok[2] = {false, false};
-        for (int s = 0; s < 2; ++s) {
-            const int k = lane + 32 * s;
+        // candidates with val > DETECTION_THRESHOLD, in slot order
+        int rows = 0;
+        for (int k0 = 0; k0 < K; k0 += NT) {
+            const int k = k0 + tid;
+            float v = 0.f;
+            bool ok = false;
             if (k < K) {
-                v[s] = a.val_k[base + k];
-                ok[s] = (double)v[s] > a.det_thr;
+                v = a.val_k[base + k];
+                ok = (double)v > a.det_thr;
             }
-        }
-        const u64 mask = ballot64(ok[0], ok[1]);
-        const int rows = __popcll(mask);
-        if (rows == 0) continue;
-        for (int s = 0; s < 2; ++s) {
-            const int k = lane + 32 * s;
-            if (ok[s]) {
-                const int r = __popcll(mask & ((1ull << k) - 1ull));
+            int total;
+            const int r = rows + thread_rank<NT>(ok, m.red(), &total);
+            if (ok) {
                 const int ind = a.ind_k[base + k];
-                S.cx[r] = ind % W;
-                S.cy[r] = ind / W;
-                S.cv[r] = v[s];
-                for (int t = 0; t < T; ++t) S.ct[r][t] = a.tag_k[(base + k) * T + t];
+                m.cx(r) = ind % W;
+                m.cy(r) = ind / W;
+                m.cv(r) = v;
+                for (int t = 0; t < T; ++t) m.ct(r)[t] = a.tag_k[(base + k) * T + t];
             }
+            rows += total;
         }
-        __syncwarp();
+        if (rows == 0) continue;
+        m.sync();
 
         if (ji == 0 || P == 0) {
             for (int r = 0; r < rows; ++r) new_or_reset(r, idx);
@@ -527,7 +631,7 @@ tag_match_wide_kernel(const MatchArgs a) {
         const int G = P < a.max_people ? P : a.max_people;
         if (a.ignore_too_much && G == a.max_people) continue;
         // running mean tag of each grouped person
-        for (int g = lane; g < G; g += 32) {
+        for (int g = tid; g < G; g += NT) {
             const int cnt = ptagn[g];
             const float* tl = ptags + (size_t)g * J * T;
             for (int t = 0; t < T; ++t) {
@@ -538,69 +642,97 @@ tag_match_wide_kernel(const MatchArgs a) {
                     sum = tl[t];
                     for (int q = 1; q < cnt; ++q) sum = __fadd_rn(sum, tl[q * T + t]);
                 }
-                S.mean[g][t] = __fdiv_rn(sum, (float)cnt);
+                m.mean(g)[t] = __fdiv_rn(sum, (float)cnt);
             }
         }
-        __syncwarp();
+        m.sync();
         const int nn = rows > G ? rows : G;
         for (int r = 0; r < nn; ++r) {
-            for (int c = lane; c < nn; c += 32) {
+            for (int c = tid; c < nn; c += NT) {
                 double cst;
                 if (r >= rows) {
                     cst = 0.0;                     // Munkres pads missing rows with 0
                 } else if (c < G) {
                     double d2 = 0.0;
                     for (int t = 0; t < T; ++t) {
-                        const double dd = __dsub_rn((double)S.ct[r][t], (double)S.mean[c][t]);
+                        const double dd = __dsub_rn((double)m.ct(r)[t], (double)m.mean(c)[t]);
                         const double sq = __dmul_rn(dd, dd);
                         d2 = (t == 0) ? sq : __dadd_rn(d2, sq);
                     }
                     const double d = sqrt(d2);
-                    S.saved[r][c] = d;
-                    cst = a.use_det_val ? __dsub_rn(__dmul_rn(rint(d), 100.0), (double)S.cv[r]) : d;
+                    m.saved(r, c) = d;
+                    cst = a.use_det_val ? __dsub_rn(__dmul_rn(rint(d), 100.0), (double)m.cv(r)) : d;
                 } else {
                     cst = 1e10;                    // reference pads columns with 1e10 when rows > cols
                 }
-                S.C[r][c] = cst;
+                m.C(r, c) = cst;
             }
         }
-        __syncwarp();
-        munkres_warp_wide(S, nn, lane);
-        __syncwarp();
+        m.sync();
+        m.munkres(nn);
+        m.sync();
         for (int r = 0; r < rows; ++r) {
-            const int c = S.star_col[r];
-            const bool accept = (c >= 0) && (c < G) && (S.saved[r][c] < a.tag_thr);
+            const int c = m.star_col(r);
+            const bool accept = (c >= 0) && (c < G) && (m.saved(r, c) < a.tag_thr);
             if (accept) {
                 const int cnt = ptagn[c];
                 float* row = ans + ((size_t)c * J + idx) * D;
-                __syncwarp();
-                if (lane == 0) {
-                    row[0] = (float)S.cx[r];
-                    row[1] = (float)S.cy[r];
-                    row[2] = S.cv[r];
+                m.sync();
+                if (tid == 0) {
+                    row[0] = (float)m.cx(r);
+                    row[1] = (float)m.cy(r);
+                    row[2] = m.cv(r);
                     ptagn[c] = cnt + 1;
                 }
-                if (lane < T) {
-                    row[3 + lane] = S.ct[r][lane];
-                    if (cnt < J) ptags[((size_t)c * J + cnt) * T + lane] = S.ct[r][lane];
+                if (tid < T) {
+                    row[3 + tid] = m.ct(r)[tid];
+                    if (cnt < J) ptags[((size_t)c * J + cnt) * T + tid] = m.ct(r)[tid];
                 }
-                __syncwarp();
+                m.sync();
             } else {
                 new_or_reset(r, idx);
             }
         }
     }
-    if (lane == 0) a.num_people[n] = P;
+    if (tid == 0) a.num_people[n] = P;
+}
+
+__global__ void __launch_bounds__(32)
+tag_match_kernel(const MatchArgs a) {
+    __shared__ MatchSmem S;
+    WarpMatcher<MatchSmem> m{S};
+    match_image(a, m);
+}
+
+__global__ void __launch_bounds__(32)
+tag_match_wide_kernel(const MatchArgs a) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    WarpMatcher<MatchSmemW> m{*reinterpret_cast<MatchSmemW*>(smem_raw)};
+    match_image(a, m);
+}
+
+__global__ void __launch_bounds__(MC_THREADS)
+tag_match_cta_kernel(const MatchArgs a) {
+    __shared__ MatchSmemC S;
+    const size_t side = (size_t)a.K * a.K;
+    CtaMatcher m{S, a.mat + 2 * side * blockIdx.x, a.mat + 2 * side * blockIdx.x + side, a.K};
+    match_image(a, m);
 }
 
 }  // namespace lp
 
 using namespace lp;
 
+static size_t match_person_bytes(int N, int J, int T, int pcap) {
+    return ((size_t)N * pcap * (sizeof(float) + sizeof(int32_t) + (size_t)J * T * sizeof(float)) + 255) / 256 * 256;
+}
+
 extern "C" size_t lp_tag_match_workspace_bytes(int N, int J, int K, int T, int pcap) {
-    (void)K;
-    if (N <= 0 || J <= 0 || T <= 0 || pcap <= 0) return 0;
-    return (size_t)N * pcap * (sizeof(float) + sizeof(int32_t) + (size_t)J * T * sizeof(float));
+    if (N <= 0 || J <= 0 || K <= 0 || T <= 0 || pcap <= 0) return 0;
+    // per-person keys, tag counts and tag lists; for K > 64 also the CTA matcher's two fp64 K x K matrices per image
+    const size_t mats = K > MW ? (size_t)N * 2 * K * K * sizeof(double) : 0;
+    return (K > MW ? match_person_bytes(N, J, T, pcap) : (size_t)N * pcap * (sizeof(float) + sizeof(int32_t) +
+                                                                             (size_t)J * T * sizeof(float))) + mats;
 }
 
 // Both entry points: W > 0 (uniform) or desc != nullptr (ragged).
@@ -610,10 +742,19 @@ static int tag_match_launch(const float* val_k, const int32_t* ind_k, const floa
                             float* ans, int32_t* num_people, void* workspace, size_t workspace_bytes, lp_stream_t stream,
                             const char* name) {
     LP_CHECK_ARG(val_k && ind_k && tag_k && joint_order && ans && num_people && workspace, "%s: null pointer", name);
-    LP_CHECK_ARG(N > 0 && J > 0 && J <= 32 && K > 0 && K <= MW && T > 0 && T < 8 && (W > 0 || desc),
-                 "%s: bad shape N=%d J=%d K=%d T=%d (J<=32, K<=64, T<8)", name, N, J, K, T);
-    LP_CHECK_ARG(max_num_people > 0 && max_num_people <= MW, "%s: max_num_people=%d out of range (1..64)", name,
-                 max_num_people);
+    // the uniform entry point keeps its K <= 64 contract; the ragged one takes K up to LP_PARSER_MAX_PEOPLE
+    if (desc)
+        LP_CHECK_ARG(N > 0 && J > 0 && J <= 32 && K > 0 && K <= LP_PARSER_MAX_PEOPLE && T > 0 && T < 8,
+                     "%s: bad shape N=%d J=%d K=%d T=%d (J<=32, K<=LP_PARSER_MAX_PEOPLE=%d, T<8)", name, N, J, K, T,
+                     LP_PARSER_MAX_PEOPLE);
+    else
+        LP_CHECK_ARG(N > 0 && J > 0 && J <= 32 && K > 0 && K <= MW && T > 0 && T < 8 && W > 0,
+                     "%s: bad shape N=%d J=%d K=%d T=%d (J<=32, K<=64, T<8; lp_tag_match_ragged_f32 takes K up to "
+                     "LP_PARSER_MAX_PEOPLE)", name, N, J, K, T);
+    const bool cta = K > MW;
+    const int max_side = cta ? K : MW;
+    LP_CHECK_ARG(max_num_people > 0 && max_num_people <= max_side,
+                 "%s: max_num_people=%d out of range (1..%d: 64, or K when K > 64)", name, max_num_people, max_side);
     LP_CHECK_ARG(pcap >= max_num_people, "%s: pcap=%d must be >= max_num_people=%d", name, pcap, max_num_people);
     LP_CHECK_ARG(det_threshold >= 0.0, "%s: detection threshold must be >= 0", name);
     const size_t need = lp_tag_match_workspace_bytes(N, J, K, T, pcap);
@@ -633,6 +774,13 @@ static int tag_match_launch(const float* val_k, const int32_t* ind_k, const floa
     a.pkey = reinterpret_cast<float*>(ws);
     a.ptagn = reinterpret_cast<int32_t*>(ws + (size_t)N * pcap * sizeof(float));
     a.ptags = reinterpret_cast<float*>(ws + (size_t)N * pcap * (sizeof(float) + sizeof(int32_t)));
+    a.mat = cta ? reinterpret_cast<double*>(ws + match_person_bytes(N, J, T, pcap)) : nullptr;
+    if (cta) {
+        LP_CHECK_ARG((reinterpret_cast<uintptr_t>(workspace) & 7) == 0, "%s: workspace must be 8-byte aligned", name);
+        tag_match_cta_kernel<<<N, MC_THREADS, 0, (cudaStream_t)stream>>>(a);
+        LP_LAUNCH_CHECK("tag_match_cta_kernel");
+        return LP_OK;
+    }
     const char* env_wide = getenv("LP_MATCH_WIDE");       // read per call: the tests flip it inside one process
     const bool force_wide = env_wide && env_wide[0] == '1';
     if (K > MM || max_num_people > MM || force_wide) {

@@ -5,10 +5,32 @@ for a whole batch on the GPU: NMS+top-K, tag matching (Munkres), adjust, scores,
 with one D2H copy of the packed result at the end.  A batch of N images equals N
 independent reference ``parse`` calls (the reference API is batch-1, SURVEY H5).
 """
+import os
+import re
+
 import numpy as np
 import torch
 
 from . import _lib
+
+
+def _header_define(name):
+    path = os.path.join(os.path.dirname(_lib.HERE), "include", "litepose_b200.h")
+    with open(path) as f:
+        return int(re.search(r"#define\s+%s\s+(\d+)" % name, f.read()).group(1))
+
+
+# the most top-K slots and matcher columns the parser kernels hold; the kernels refuse more with LP_ERR_BAD_ARG
+PARSER_MAX_PEOPLE = _header_define("LP_PARSER_MAX_PEOPLE")
+
+
+def check_max_people(max_num_people):
+    """MAX_NUM_PEOPLE is K, the top-K slots per joint and the side of the matcher's cost matrices; the kernels take up
+    to LP_PARSER_MAX_PEOPLE (include/litepose_b200.h)."""
+    bound = PARSER_MAX_PEOPLE
+    if int(max_num_people) > bound:
+        raise ValueError("MAX_NUM_PEOPLE=%d exceeds LP_PARSER_MAX_PEOPLE=%d, the most top-K slots and matcher columns "
+                         "the parser kernels hold" % (int(max_num_people), bound))
 
 
 class DeviceParser(object):
@@ -19,8 +41,7 @@ class DeviceParser(object):
                              % (nms_kernel, nms_padding))
         if detection_threshold < 0:
             raise ValueError("DETECTION_THRESHOLD must be >= 0 (slots with val <= 0 are canonicalised)")
-        if max_num_people > 64:
-            raise ValueError("MAX_NUM_PEOPLE > 64 is not supported by the warp-wide matcher (two columns per lane)")
+        check_max_people(max_num_people)
         self.lib = _lib.load()
         self.J = int(num_joints)
         self.K = int(max_num_people)
@@ -31,6 +52,9 @@ class DeviceParser(object):
         self.joint_order = [int(v) for v in joint_order[: self.J]]
         self.nms_kernel = int(nms_kernel)
         self.pcap = self.J * self.K          # worst case: every candidate founds a person
+        # K > 64: the uniform top-K and matching entry points keep their K <= 64 contract, so a uniform batch goes
+        # through the ragged ones as N equal map descriptors (per image the same results)
+        self.uniform_as_ragged = self.K > 64
         self._bufs = {}
         self._jo = {}
 
@@ -47,10 +71,22 @@ class DeviceParser(object):
                 "ans": torch.empty((n, pcap, J, 3 + t), dtype=f32, device=dev),
                 "num": torch.empty((n,), dtype=i32, device=dev),
                 "scores": torch.empty((n, pcap), dtype=f32, device=dev),
-                "ws_topk": torch.empty(max(1, lib.lp_nms_topk_workspace_bytes(n, J, h, w, K)), dtype=u8, device=dev),
+                "ws_topk": torch.empty(max(1, lib.lp_nms_topk_workspace_bytes(n, J, h, w, K)), dtype=u8, device=dev)
+                if not self.uniform_as_ragged else None,
                 "ws_match": torch.empty(max(1, lib.lp_tag_match_workspace_bytes(n, J, K, t, pcap)), dtype=u8, device=dev),
                 "ws_ref": torch.empty(max(1, lib.lp_adjust_refine_workspace_bytes(n, J, pcap)), dtype=u8, device=dev),
             }
+            if self.uniform_as_ragged:
+                from .mixed import MAP_DESC
+                hw = np.ascontiguousarray(np.tile([[h, w]], (n, 1)), np.int32)
+                desc = np.zeros(n, MAP_DESC)
+                desc["h"], desc["w"] = h, w
+                desc["det_offset"] = np.arange(n) * (J * h * w)
+                desc["tag_offset"] = np.arange(n) * (J * h * w * t)
+                b["hw"] = hw
+                b["desc"] = torch.from_numpy(desc.view(np.uint8)).to(dev)
+                b["ws_topk"] = torch.empty(max(1, lib.lp_nms_topk_ragged_workspace_bytes(n, hw.ctypes.data, J, K)),
+                                           dtype=u8, device=dev)
             self._bufs[key] = b
         if dev not in self._jo:
             self._jo[dev] = torch.tensor(self.joint_order, dtype=torch.int32, device=dev)
@@ -66,10 +102,32 @@ class DeviceParser(object):
         det, tag = det.contiguous(), tag.contiguous()
         b, _ = self._buffers(det.device, n, h, w, t)
         s = torch.cuda.current_stream().cuda_stream
+        if self.uniform_as_ragged:
+            _lib.check(self.lib.lp_nms_topk_ragged_f32(
+                det.data_ptr(), tag.data_ptr(), n, b["hw"].ctypes.data, b["desc"].data_ptr(), j, t, self.nms_kernel,
+                self.K, float(min_value), b["val_k"].data_ptr(), b["ind_k"].data_ptr(), b["tag_k"].data_ptr(),
+                b["ws_topk"].data_ptr(), b["ws_topk"].numel(), s), "lp_nms_topk_ragged_f32")
+            return b["val_k"], b["ind_k"], b["tag_k"]
         _lib.check(self.lib.lp_nms_topk_f32(det.data_ptr(), tag.data_ptr(), n, j, h, w, t, self.nms_kernel, self.K,
                                             float(min_value), b["val_k"].data_ptr(), b["ind_k"].data_ptr(), b["tag_k"].data_ptr(),
                                             b["ws_topk"].data_ptr(), b["ws_topk"].numel(), s), "lp_nms_topk_f32")
         return b["val_k"], b["ind_k"], b["tag_k"]
+
+    def match_device(self, dev, n, h, w, t):
+        """tag matching on the top-K buffers of the (n, h, w, t) shape left by top_k_device -> device (ans, num)"""
+        b, jo = self._buffers(dev, n, h, w, t)
+        s = torch.cuda.current_stream().cuda_stream
+        j = self.J
+        tail = (jo.data_ptr(), self.det_thr, self.tag_thr, self.use_det_val, self.ignore_too_much, self.K, self.pcap,
+                b["ans"].data_ptr(), b["num"].data_ptr(), b["ws_match"].data_ptr(), b["ws_match"].numel(), s)
+        if self.uniform_as_ragged:
+            _lib.check(self.lib.lp_tag_match_ragged_f32(b["val_k"].data_ptr(), b["ind_k"].data_ptr(),
+                                                        b["tag_k"].data_ptr(), n, j, self.K, t, b["desc"].data_ptr(),
+                                                        *tail), "lp_tag_match_ragged_f32")
+        else:
+            _lib.check(self.lib.lp_tag_match_f32(b["val_k"].data_ptr(), b["ind_k"].data_ptr(), b["tag_k"].data_ptr(),
+                                                 n, j, self.K, t, w, *tail), "lp_tag_match_f32")
+        return b["ans"], b["num"]
 
     def run(self, det, tag, adjust=True, refine=True):
         """det [N,J,H,W] fp32 CUDA, tag [N,J,H,W,T] fp32 CUDA -> device (ans, num_people, scores)."""
@@ -84,11 +142,7 @@ class DeviceParser(object):
             b, jo = self._buffers(det.device, n, h, w, t)
             s = torch.cuda.current_stream().cuda_stream
             self.top_k_device(det, tag, self.det_thr)
-            _lib.check(self.lib.lp_tag_match_f32(
-                b["val_k"].data_ptr(), b["ind_k"].data_ptr(), b["tag_k"].data_ptr(), n, j, self.K, t, w,
-                jo.data_ptr(), self.det_thr, self.tag_thr, self.use_det_val, self.ignore_too_much, self.K,
-                self.pcap, b["ans"].data_ptr(), b["num"].data_ptr(), b["ws_match"].data_ptr(),
-                b["ws_match"].numel(), s), "lp_tag_match_f32")
+            self.match_device(det.device, n, h, w, t)
             _lib.check(self.lib.lp_adjust_refine_f32(
                 det.data_ptr(), tag.data_ptr(), n, j, h, w, t, self.pcap, b["ans"].data_ptr(), b["num"].data_ptr(),
                 b["scores"].data_ptr(), 1 if adjust else 0, 1 if refine else 0, b["ws_ref"].data_ptr(),

@@ -17,7 +17,7 @@ import torch
 
 from . import _lib
 from .config import flip_index_for
-from .parser import DeviceParser
+from .parser import DeviceParser, check_max_people
 
 
 class PlantedCrowd(object):
@@ -190,6 +190,7 @@ class LitePosePipeline(object):
             bad("WITH_AE_LOSS / TEST.WITH_AE other than (True, False)")
         if int(cfg.LOSS.NUM_STAGES) != 2:
             bad("LOSS.NUM_STAGES=%r" % (cfg.LOSS.NUM_STAGES,))
+        check_max_people(cfg.DATASET.MAX_NUM_PEOPLE)
 
     @staticmethod
     def _validate_fast_cfg(cfg):
