@@ -48,6 +48,29 @@ def image_shapes(images):
     return shapes
 
 
+def multi_scale_sizes(shape, scales, input_size):
+    """Per scale of ``scales`` (the pipeline's order, largest first) for an image of ``shape`` (h, w): the network
+    input size (h_s, w_s) and the (center, scale) get_multi_scale_size gives.  Returns (key, [(center, scale)]); the
+    key, the tuple of per-scale sizes, names the image's size group."""
+    probe = np.broadcast_to(np.uint8(0), (int(shape[0]), int(shape[1]), 3))     # only its shape is read
+    smin = min(scales)
+    sizes, cs = [], []
+    for s in scales:
+        (w_r, h_r), c, sc = tf.get_multi_scale_size(probe, input_size, s, smin)
+        sizes.append((h_r, w_r))
+        cs.append((c, sc))
+    return tuple(sizes), cs
+
+
+def group_order(keys):
+    """Arena order of a list whose images have the size-group keys ``keys``: groups in first-appearance order, caller
+    order inside a group.  A list already in this order keeps it."""
+    groups = {}
+    for i, k in enumerate(keys):
+        groups.setdefault(k, []).append(i)
+    return [i for g in groups.values() for i in g]
+
+
 class Group(object):
     """One size group: ``images`` (caller indices, in arena order), per-scale input sizes ``in_hw[s]`` = (h, w), the
     common det / tag size ``det_hw`` and the group's first position in the arenas ``start``."""
@@ -72,31 +95,22 @@ class MixedPlan(object):
 
     def __init__(self, shapes, scales, input_size, project, J, T):
         scales = list(scales)                        # the pipeline's order: largest first
-        smin = min(scales)
         self.scales = scales
         self.shapes = list(shapes)
         self.J, self.T = int(J), int(T)
         n = len(shapes)
-        per = []
+        per = [multi_scale_sizes(s, scales, input_size) for s in shapes]
+        self.keys = [per[i][0] for i in range(n)]
+        self.order = group_order(self.keys)
         groups = {}
-        for i, (h, w) in enumerate(shapes):
-            probe = np.empty((h, w, 3), np.uint8)
-            sizes, cs = [], []
-            for s in scales:
-                (w_r, h_r), c, sc = tf.get_multi_scale_size(probe, input_size, s, smin)
-                sizes.append((h_r, w_r))
-                cs.append((c, sc))
-            key = tuple(sizes)
-            per.append((key, cs))
-            g = groups.get(key)
-            if g is None:
-                g = groups[key] = Group(key, scales)
-            g.images.append(i)
+        for i in self.order:
+            k = self.keys[i]
+            if k not in groups:
+                groups[k] = Group(k, scales)
+            groups[k].images.append(i)
         self.groups = list(groups.values())
-        self.order = [i for g in self.groups for i in g.images]
         self.pos = np.empty(n, np.int64)                # caller index -> arena position
         self.pos[self.order] = np.arange(n)
-        self.keys = [per[i][0] for i in range(n)]
         self.center_scale = [per[i][1] for i in range(n)]     # caller order, per scale (center, scale)
         self.src_off = np.zeros(n + 1, np.int64)
         self.in_off = {s: np.zeros(n + 1, np.int64) for s in scales}

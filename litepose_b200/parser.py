@@ -149,8 +149,9 @@ class DeviceParser(object):
                 b["ws_ref"].numel(), s), "lp_adjust_refine_f32")
         return b["ans"], b["num"], b["scores"]
 
-    def _ragged_buffers(self, dev, n, t, ws_topk, ws_match, ws_ref):
-        """Grow-only buffers of run_ragged: one set, sized for the largest batch seen (not one per composition)."""
+    def _ragged_buffers(self, dev, n, t, ws_topk, ws_match, ws_ref, outs=None):
+        """Grow-only buffers of run_ragged: one set, sized for the largest batch seen (not one per composition).  The
+        results (ans, num, scores) grow in ``outs`` instead when the caller passes its own dict."""
         J, K, pcap = self.J, self.K, self.pcap
         sizes = {"val_k": (n * J * K, torch.float32), "ind_k": (n * J * K, torch.int32),
                  "tag_k": (n * J * K * t, torch.float32), "ans": (n * pcap * J * (3 + t), torch.float32),
@@ -159,9 +160,10 @@ class DeviceParser(object):
         bufs = self._bufs.setdefault(("ragged", dev), {})
         out = {}
         for name, (numel, dtype) in sizes.items():
-            b = bufs.get(name)
+            home = outs if outs is not None and name in ("ans", "num", "scores") else bufs
+            b = home.get(name)
             if b is None or b.numel() < numel:
-                b = bufs[name] = torch.empty(max(int(numel), 1), dtype=dtype, device=dev)
+                b = home[name] = torch.empty(max(int(numel), 1), dtype=dtype, device=dev)
             out[name] = b[:max(int(numel), 1)]
         if dev not in self._jo:
             self._jo[dev] = torch.tensor(self.joint_order, dtype=torch.int32, device=dev)
@@ -175,20 +177,21 @@ class DeviceParser(object):
                 int(self.lib.lp_tag_match_workspace_bytes(n, self.J, self.K, t, self.pcap)),
                 int(self.lib.lp_adjust_refine_workspace_bytes(n, self.J, self.pcap)))
 
-    def run_ragged(self, det, tag, hw, desc, t, adjust=True, refine=True):
+    def run_ragged(self, det, tag, hw, desc, t, adjust=True, refine=True, outs=None):
         """The parse of run() on a det / tag arena of differently sized maps: image i's [J,h_i,w_i] det block and
         [J,h_i,w_i,T] tag block sit at the offsets of ``desc`` (device pointer to N lp_map_desc_t,
         litepose_b200.mixed.MAP_DESC); ``hw`` [N,2] int32 host array = the same sizes.  One ragged chain (NMS/top-K, tag
         matching, adjust/scores/refine) for the whole batch.  Per image the results equal, bit for bit, run() on that
         image alone.  Returns device (ans [N,pcap,J,3+T], num [N], scores [N,pcap]) in grow-only buffers, valid until
-        the next ragged call."""
+        the next ragged call with the same ``outs``: a caller's dict that owns the result buffers (None: the parser's
+        own).  The top-K lists and workspaces are shared by every call, in stream order."""
         if not det.is_cuda:
             raise RuntimeError("litepose_b200 parser runs on CUDA tensors only (no CPU fallback)")
         hw = np.ascontiguousarray(hw, np.int32)
         n, j = hw.shape[0], self.J
         ws = self.workspace_bytes_ragged(hw, t)
         with torch.cuda.device(det.device):
-            b, jo = self._ragged_buffers(det.device, n, t, *ws)
+            b, jo = self._ragged_buffers(det.device, n, t, *ws, outs=outs)
             s = torch.cuda.current_stream().cuda_stream
             _lib.check(self.lib.lp_nms_topk_ragged_f32(
                 det.data_ptr(), tag.data_ptr(), n, hw.ctypes.data, desc, j, t, self.nms_kernel, self.K, self.det_thr,

@@ -106,6 +106,18 @@ def unpack_fast_payload(host, M, J):
     return out
 
 
+class ImagesTicket(object):
+    """Ticket of LitePosePipeline.submit_images: which list slot holds the list, and the submission it belongs to.  Only
+    collect_images takes it (the tickets of submit() are slot numbers)."""
+    __slots__ = ("owner", "slot", "serial")
+
+    def __init__(self, owner, slot, serial):
+        self.owner, self.slot, self.serial = owner, slot, serial
+
+    def __repr__(self):
+        return "ImagesTicket(slot=%d, serial=%d)" % (self.slot, self.serial)
+
+
 class LitePosePipeline(object):
     def __init__(self, model, cfg, use_graphs=True, keep=64, grouping="ae"):
         """model: litepose_b200 drop-in LitePose on a CUDA device (eval).
@@ -281,12 +293,13 @@ class LitePosePipeline(object):
             o, f = self._network_part(side, xs[s], arena=arena)
             self._glue(o, f, det, tag, plant, i)
 
-    def _parse(self, det, tag, packed, trans, fb=None, ragged=None):
+    def _parse(self, det, tag, packed, trans, fb=None, ragged=None, outs=None):
         """The grouping mode's device parser, get_final_preds (``trans``: device pointer to [N,6] float64 matrices, or
         None) and payload pack on det / tag -> ``packed``.  Uniform maps: det [N,J,H,W], tag [N,1|J,H,W,T]; ragged
-        arena: ``ragged`` = (hw [N,2] host int32, device pointer to the lp_map_desc_t of the maps).  ``fb``: the fast
-        grouping's buffers (_fast_buffers).  Returns the ae parser's own buffers (ans, num, scores; capacity J*K
-        persons, valid until its next run) for fetch_overflow; None with grouping="fast"."""
+        arena: ``ragged`` = (hw [N,2] host int32, device pointer to the lp_map_desc_t of the maps), ``outs`` the dict
+        that owns the ragged parser's results (DeviceParser.run_ragged).  ``fb``: the fast grouping's buffers
+        (_fast_buffers).  Returns the ae parser's own buffers (ans, num, scores; capacity J*K persons, valid until its
+        next run) for fetch_overflow; None with grouping="fast"."""
         J, T = self.params.num_joints, self.T
         hw, desc = ragged if ragged is not None else (None, None)
         n = det.shape[0] if ragged is None else len(hw)
@@ -308,7 +321,7 @@ class LitePosePipeline(object):
                                               fb["ind"].data_ptr(), f["jo"].data_ptr(), n, J, M, f["tag_thr"],
                                               num.data_ptr(), ans.data_ptr(), fb["status"].data_ptr(), s), "lp_assign_f32")
         elif ragged is not None:
-            ans, num, scores = full = self.parser.run_ragged(det, tag, hw, desc, T, self.adjust, self.refine)
+            ans, num, scores = full = self.parser.run_ragged(det, tag, hw, desc, T, self.adjust, self.refine, outs)
         else:
             if self.tag_shared:
                 # MODEL.TAG_PER_JOINT off: the one tag map serves every joint (group.py:150-152); the parser kernels
@@ -575,27 +588,52 @@ class LitePosePipeline(object):
                 self.set_final_preds(prev[0], prev[1])
 
     # -- mixed batches: differently sized images in one call --------------------------------------------------------
-    def _grow(self, name, numel, dtype, pinned=False):
+    def _grow(self, name, numel, dtype, pinned=False, bufs=None):
         """Grow-only buffer of the mixed path (``numel`` elements at least): its size follows the largest batch served,
-        not the number of batch compositions."""
-        buf = self._mixed_bufs.get(name)
+        not the number of batch compositions.  ``bufs``: the dict it lives in, a list slot's own buffers (_mixed_init),
+        or by default the buffers every list shares."""
+        bufs = self._mixed_bufs if bufs is None else bufs
+        buf = bufs.get(name)
         if buf is None or buf.numel() < numel or buf.dtype != dtype:
             if pinned:
                 buf = torch.empty(max(int(numel), 1), dtype=dtype).pin_memory()
             else:
                 buf = torch.empty(max(int(numel), 1), dtype=dtype, device=self.device)
-            self._mixed_bufs[name] = buf
+            bufs[name] = buf
         return buf[:numel]
 
-    def infer_mixed(self, images, mean=(0.485, 0.456, 0.406), std=(0.229, 0.224, 0.225), half=True, plant=None):
-        """infer_images for a list of uint8 [H_i,W_i,3] images of any sizes.  Per image the result equals, bit for bit,
-        infer_images(image[None]); the list comes back in the caller's order.  The images are grouped by their per-scale
-        network sizes (litepose_b200.mixed.MixedPlan).  Once per batch: one H2D copy of the packed images and
-        descriptors, per scale ONE ragged warp launch (lp_warp_affine_normalize_ragged_u8) into the input arena of that
+    def _mixed_init(self):
+        """State of the list form, made on first use.  Every list shares, in stream order (each list's device work waits
+        for the previous list's, ``_mixed_tail``, whatever stream that ran on): the input, det / tag and fast-grouping
+        arenas (``_mixed_bufs``), the engine's arena plans and the ragged parser's top-K lists and workspaces - only
+        device work reads them.  A list SLOT owns what is read after the list's device work has been queued, until its
+        result is on the host: the pinned and device staging (images, descriptors, final-pred matrices), the payload
+        rows, the pinned host rows and the ragged parser's results (read by fetch_overflow).  The blocking list form has
+        one slot, submit_images two."""
+        if hasattr(self, "_mixed_bufs"):
+            return
+        dev = self.device
+        self._mixed_bufs = {}
+        self._mixed_side = torch.cuda.Stream(device=dev)
+        self._mixed_tail = None
+        self._mixed_sync = self._list_slot()
+        self._lists = {"slots": [self._list_slot(), self._list_slot()], "serial": 0,
+                       "copy": torch.cuda.Stream(device=dev), "res": torch.cuda.Stream(device=dev)}
+
+    @staticmethod
+    def _list_slot():
+        return {"bufs": {}, "parser": {}, "done": None, "busy": False, "serial": None}
+
+    def _mixed_enqueue(self, images, mean, std, half, plant, slot, copy=None, rows=None):
+        """The device work of one mixed list, queued on the current stream without synchronising the host.  Once per
+        list: the images (arena order), descriptors and final-pred matrices are packed into ``slot``'s pinned staging
+        buffer and leave in ONE H2D copy (on the stream ``copy`` when given, so that it overlaps device work already
+        queued); per scale ONE ragged warp launch (lp_warp_affine_normalize_ragged_u8) into the input arena of that
         scale; per size group the network passes and the glue on the existing kernels (arena plans of the engine: their
         activation memory is shared by every group size), writing the group's slice of the det / tag arena; then ONE
-        ragged parser chain over the whole arena, one get_final_preds launch with per-image matrices, one payload pack
-        and one D2H copy.  Launches run eagerly (no CUDA graph: the composition changes from batch to batch)."""
+        ragged parser chain over the whole arena into ``slot``'s result buffers, one get_final_preds launch with
+        per-image matrices and one payload pack into the first N of ``slot``'s ``rows`` (default N) payload rows, in
+        arena order.  Returns the list's record (plan, payload, parser results) for _fetch / collect_images."""
         import numpy as np
         from .mixed import MixedPlan, image_shapes
         shapes = image_shapes(images)
@@ -604,9 +642,8 @@ class LitePosePipeline(object):
             raise ValueError("infer_images: %d plant entries for %d images" % (len(plant), n))
         J, T = self.params.num_joints, self.T
         mp = MixedPlan(shapes, self.scales, int(self.cfg.DATASET.INPUT_SIZE), self.project, J, T)
-        if not hasattr(self, "_mixed_bufs"):
-            self._mixed_bufs = {}
-            self._mixed_side = torch.cuda.Stream(device=self.device)
+        self._mixed_init()
+        own = slot["bufs"]
         in_dtype = torch.float16 if half else torch.float32
         # (1) one pinned staging buffer: the images (arena order) followed by the descriptors and final-pred matrices
         descs = [mp.warp_desc(s).view(np.uint8) for s in self.scales]
@@ -618,7 +655,7 @@ class LitePosePipeline(object):
         for b in blobs:
             offs.append(o)
             o = (o + b.size + 255) // 256 * 256
-        host = self._grow("stage", o, torch.uint8, pinned=True)
+        host = self._grow("stage", o, torch.uint8, pinned=True, bufs=own)
         hnp = host.numpy()
         dev_imgs = []
         for p, i in enumerate(mp.order):
@@ -630,14 +667,29 @@ class LitePosePipeline(object):
                 hnp[a:b] = (im.contiguous().numpy() if torch.is_tensor(im) else np.ascontiguousarray(im)).reshape(-1)
         for b, off in zip(blobs, offs):
             hnp[off:off + b.size] = b
-        d = self._grow("stage_dev", o, torch.uint8)
-        d.copy_(host, non_blocking=True)
+        main = torch.cuda.current_stream()
+        if self._mixed_tail is not None:
+            main.wait_event(self._mixed_tail)
+        if copy is None:
+            d = self._grow("stage_dev", o, torch.uint8, bufs=own)
+            d.copy_(host, non_blocking=True)
+        else:
+            with torch.cuda.stream(copy):
+                # allocated from the copy stream's pool: a block the current stream has just freed may still be read by
+                # work queued there, which this copy does not wait for
+                d = self._grow("stage_dev", o, torch.uint8, bufs=own)
+                if slot["done"] is not None:
+                    copy.wait_event(slot["done"])        # this slot's previous list has read its staging
+                d.copy_(host, non_blocking=True)
+                h2d = torch.cuda.Event()
+                h2d.record(copy)
+            main.wait_event(h2d)
         for a, b, im in dev_imgs:                    # images already on the device: one device copy each
             d[a:b].copy_(im.reshape(-1))
         # (2) per scale one ragged warp + ToTensor + Normalize into the scale's input arena
         mean_a, std_a = np.asarray(mean, np.float32), np.asarray(std, np.float32)
         xs_arena = {}
-        stream = torch.cuda.current_stream().cuda_stream
+        stream = main.cuda_stream
         for k, s in enumerate(self.scales):
             xa = self._grow("x%d" % k, int(mp.in_off[s][-1]), in_dtype)
             mh, mw = mp.max_in_hw(s)
@@ -671,18 +723,147 @@ class LitePosePipeline(object):
                 tag_full[:, :1].copy_(tag)          # the peak finder reads the shared map as plane 0 of the image's block
             elif self.tag_shared:
                 tag_full.copy_(tag.expand(-1, J, -1, -1, -1))
-        # (4) once per batch: ragged parser, get_final_preds, payload, D2H
+        # (4) once per list: ragged parser, get_final_preds, payload
         hw = np.ascontiguousarray(mp.det_hw, np.int32)
         fb = None
         if self.grouping == "fast":
             fb = self._fast_buffers(n, J, lambda k, shape, dt: self._grow("fast_" + k, int(np.prod(shape)), dt).view(shape))
+        width, rows = self.width, n if rows is None else rows
+        packed = self._grow("packed", rows * width, torch.float32, bufs=own).view(rows, width)
+        full = self._parse(det_a, tag_a, packed[:n], d.data_ptr() + offs[-1], fb, (hw, d.data_ptr() + offs[-2]),
+                           slot["parser"])
+        done = torch.cuda.Event()
+        done.record(main)
+        slot["done"] = self._mixed_tail = done
+        # the caller's images and plant hooks stay referenced until the result has been read
+        return {"plan": mp, "det": det_a, "tag": tag_a, "inputs": xs_arena, "packed": packed, "full": full, "n": n,
+                "refs": (images, plant)}
+
+    def infer_mixed(self, images, mean=(0.485, 0.456, 0.406), std=(0.229, 0.224, 0.225), half=True, plant=None):
+        """infer_images for a list of uint8 [H_i,W_i,3] images of any sizes.  Per image the result equals, bit for bit,
+        infer_images(image[None]); the list comes back in the caller's order.  The images are grouped by their per-scale
+        network sizes (litepose_b200.mixed.MixedPlan); _mixed_enqueue queues the list's device work, then ONE D2H copy
+        and a synchronise.  Launches run eagerly (no CUDA graph: the composition changes from batch to batch)."""
+        self._mixed_init()
+        sl = self._mixed_sync
+        rec = self._last_mixed = self._mixed_enqueue(images, mean, std, half, plant, sl)
+        n = rec["n"]
+        rec["host"] = self._grow("host", n * self.width, torch.float32, pinned=True, bufs=sl["bufs"]).view(n, self.width)
+        res = self._fetch(rec)
+        return [res[int(p)] for p in rec["plan"].pos]
+
+    # -- asynchronous list API: two mixed lists in flight ---------------------------------------------------------------
+    def submit_images(self, images, plant=None, group=None, dst=0, plan=None, mean=(0.485, 0.456, 0.406),
+                      std=(0.229, 0.224, 0.225), half=True):
+        """Asynchronous form of infer_images on a list of uint8 [H_i,W_i,3] images of any sizes (``plant``: one batch-1
+        PlantedCrowd or None per image).  Returns an ImagesTicket; ``collect_images(ticket)`` returns exactly what
+        infer_images(images) returns.  Nothing here synchronises the host: the list is staged in its slot's pinned
+        buffer and copied on a copy stream, so that the staging and H2D copy of list i+1 overlap the device work of list
+        i; the device work is queued on the current stream, and the payload rows leave through the result stream.  At
+        most two lists may be outstanding (a third submit raises); their tickets are apart from those of submit().
+
+        ``group`` (a torch.distributed process group of one rank per GPU): ``images`` is this rank's shard of a list
+        split by ``plan`` = litepose_b200.dist.plan_shards(shapes, cfg, world), the same on every rank, in the order of
+        plan.indices[rank].  Every rank's payload, padded to plan.rows rows, is gathered on rank ``dst`` with ONE NCCL
+        gather on the result stream and leaves that rank in ONE device->host copy.  The gathered payload carries
+        ``keep`` persons per image: collect_images raises for an image with more (use a larger ``keep``)."""
+        import torch.distributed as dist
+        self._mixed_init()
+        world, rank = 1, 0
+        if group is not None:
+            if plan is None:
+                raise ValueError("submit_images(group=...): pass the shard plan (litepose_b200.dist.plan_shards)")
+            world, rank = dist.get_world_size(group), dist.get_rank(group)
+            if plan.world != world:
+                raise ValueError("submit_images: a plan over %d ranks for a group of %d" % (plan.world, world))
+            mine = [plan.shapes[i] for i in plan.indices[rank]]
+            from .mixed import image_shapes
+            got = image_shapes(images) if len(images) else []
+            if got != mine:
+                raise ValueError("submit_images: rank %d's images must be the list's images plan.indices[%d], in that "
+                                 "order (sizes %r, expected %r)" % (rank, rank, got, mine))
+        a = self._lists
+        free = [k for k, s in enumerate(a["slots"]) if not s["busy"]]
+        if not free:
+            raise RuntimeError("LitePosePipeline.submit_images: two lists are already in flight - collect_images() one "
+                               "first")
+        k = free[0]
+        sl = a["slots"][k]
         width = self.width
-        packed = self._grow("packed", n * width, torch.float32).view(n, width)
-        full = self._parse(det_a, tag_a, packed, d.data_ptr() + offs[-1], fb, (hw, d.data_ptr() + offs[-2]))
-        self._last_mixed = {"plan": mp, "det": det_a, "tag": tag_a, "inputs": xs_arena, "packed": packed, "full": full,
-                            "host": self._grow("host", n * width, torch.float32, pinned=True).view(n, width)}
-        res = self._fetch(self._last_mixed)
-        return [res[int(p)] for p in mp.pos]
+        rows = plan.rows if group is not None else None
+        if len(images) or group is None:
+            rec = self._mixed_enqueue(images, mean, std, half, plant, sl, copy=a["copy"], rows=rows)
+            if group is not None and rec["plan"].order != list(range(rec["n"])):
+                # the gathered rows are in arena order; dst maps them back through plan.indices alone
+                raise ValueError("submit_images: plan.indices[%d] is not in the arena order of this pipeline's sizes "
+                                 "(a plan made for another TEST.SCALE_FACTOR or INPUT_SIZE)" % rank)
+        else:
+            # an empty shard still takes part in the gather (its rows are padding)
+            rec = {"plan": None, "n": 0, "full": None, "refs": None,
+                   "packed": self._grow("packed", rows * width, torch.float32, bufs=sl["bufs"]).view(rows, width)}
+            done = torch.cuda.Event()
+            done.record(torch.cuda.current_stream())
+            sl["done"] = done
+        own = sl["bufs"]
+        res = a["res"]
+        gathered = None
+        if group is None:
+            host = self._grow("host", rec["n"] * width, torch.float32, pinned=True, bufs=own).view(rec["n"], width)
+        elif rank == dst:
+            host = self._grow("host", world * rows * width, torch.float32, pinned=True, bufs=own).view(world, rows, width)
+            if world > 1:
+                gathered = self._grow("gather", world * rows * width, torch.float32, bufs=own).view(world, rows, width)
+        else:
+            host = None
+        with torch.cuda.stream(res):
+            res.wait_event(sl["done"])
+            if group is not None and world > 1:
+                from .dist import gather_rows
+                gather_rows(rec["packed"], gathered, dst=dst, group=group)
+                if gathered is not None:
+                    host.copy_(gathered, non_blocking=True)
+            elif host is not None:
+                host.view(-1, width).copy_(rec["packed"], non_blocking=True)
+            d2h = torch.cuda.Event()
+            d2h.record(res)
+        rec["host"] = host
+        a["serial"] += 1
+        sl.update(busy=True, serial=a["serial"], rec=rec, d2h=d2h, dist=(group is not None, rank, dst, plan))
+        return ImagesTicket(self, k, a["serial"])
+
+    def collect_images(self, ticket):
+        """Wait for the list behind ``ticket`` (submit_images).  Without a group: the list over images, in the caller's
+        order, that infer_images returns; an ae image with more than ``keep`` persons is read in full from the slot's
+        parser buffers.  With a group: on ``dst`` the per-rank lists (rank r's in the order of plan.indices[r];
+        litepose_b200.dist.merge_shards restores the caller's order), None on the other ranks."""
+        if not isinstance(ticket, ImagesTicket):
+            raise TypeError("collect_images: a ticket of submit_images expected, got %r" % (ticket,))
+        a = getattr(self, "_lists", None)
+        sl = a["slots"][ticket.slot] if a is not None and ticket.owner is self else None
+        if sl is None or not sl["busy"] or sl["serial"] != ticket.serial:
+            raise RuntimeError("LitePosePipeline.collect_images: %r is not in flight" % (ticket,))
+        sl["d2h"].synchronize()
+        rec = sl.pop("rec")
+        sl["busy"] = False
+        grouped, rank, dst, plan = sl["dist"]
+        if not grouped:
+            res = self._decode(rec["host"], rec)
+            return [res[int(p)] for p in rec["plan"].pos]
+        if rank != dst:
+            return None
+        from .dist import split_rows
+        out = []
+        for r, host in enumerate(split_rows(rec["host"], plan)):
+            if self.grouping == "ae":
+                over = (host[:, -1] > self.keep).nonzero().flatten().tolist()
+                if over:
+                    q = over[0]
+                    raise _lib.LitePoseError(
+                        "image %d of the list (rank %d's image %d) holds %d persons but the gathered payload carries "
+                        "keep=%d: construct the pipeline with a larger keep (up to %d)"
+                        % (plan.indices[r][q], r, q, int(host[q, -1]), self.keep, self.parser.pcap))
+            out.append(self._decode(host))
+        return out
 
     # -- asynchronous end-to-end API: two steps in flight -----------------------------------------
     def submit(self, frames_pinned, plant=None, group=None, dst=0):
