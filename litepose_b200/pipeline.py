@@ -496,13 +496,20 @@ class LitePosePipeline(object):
         # the state of the last step_device / step_device_multiscale call: its det / tag / packed stay readable there
         # until the next call
         st = self._last_state = self._get_state(n, s_h, s_w, x_dev.dtype, plant)
-        ov = st.get("ov")
-        if ov is not None:
-            # det / tag / packed are shared with buffer set 0 of the overlapped form: an overlapped step that is still
-            # running on the parser stream must finish before this stream overwrites them
+        main = torch.cuda.current_stream()
+        for other in self._state.values():
+            ov = other.get("ov")
+            if ov is None:
+                continue
+            # an overlapped step still queued on a parser stream reads buffers this step overwrites: the engine's
+            # buffer set 0 and the parser's buffers (shared by every state of the same shapes), and this state's det /
+            # tag (its buffer set 0)
             for ev in ov["P_done"]:
                 if ev is not None:
-                    torch.cuda.current_stream().wait_event(ev)
+                    main.wait_event(ev)
+            if other is st and ov["consumer_done"][0] is not None:
+                # st["packed"] is buffer set 0's payload: submit() may not have copied it out on its result stream yet
+                main.wait_event(ov["consumer_done"][0])
         if not self.use_graphs:
             self._device_step(st, x_dev)
             return st["packed"]
@@ -873,7 +880,10 @@ class LitePosePipeline(object):
         stream (D2H of step i overlaps the compute of step i+1; with ``group`` - a torch.distributed process group of
         one rank per GPU - the slot is first gathered on rank ``dst`` with ONE NCCL gather and leaves that rank in
         ONE device->host copy).  At most two tickets may be outstanding.  An image with more persons than ``keep``
-        makes collect() raise (never clipped): use the blocking step(), or a larger ``keep``."""
+        makes collect() raise (never clipped): use the blocking step(), or a larger ``keep``.
+
+        ``frames_pinned`` is read by the copy stream after this call has returned, and is not copied here: the caller
+        must leave it unchanged until collect(ticket) has returned."""
         import torch.distributed as dist
         n, _, s_h, s_w = frames_pinned.shape
         main = torch.cuda.current_stream()
