@@ -1,4 +1,5 @@
-"""ctypes binding of the C-ABI shared library (include/litepose_b200.h).
+"""ctypes binding of the C-ABI shared library (include/litepose_b200.h, and include/litepose_b200_train.h for the
+training kernels).
 
 The CUDA library is the product: there is no Python/PyTorch fallback.  Importing
 this module never compiles anything; ``load()`` raises ``LitePoseLibraryError`` if the
@@ -14,6 +15,7 @@ LIB_PATH = os.path.join(HERE, "_C", "liblitepose_b200.so")
 
 LP_OK = 0
 ACT_NONE, ACT_RELU, ACT_RELU6 = 0, 1, 2
+LP_DT_F32, LP_DT_F16 = 0, 1
 
 
 class LitePoseLibraryError(RuntimeError):
@@ -91,6 +93,14 @@ SIGNATURES = {
     "lp_pack_fast_payload_f32": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp]),
 }
 
+# every symbol declared in include/litepose_b200_train.h (the same library)
+TRAIN_SIGNATURES = {
+    "lp_dw_nchw_fwd": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "lp_dw_nchw_dgrad": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "lp_dw_nchw_wgrad_workspace_bytes": (_sz, [_i, _i, _i, _i, _i, _i]),
+    "lp_dw_nchw_wgrad": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _sz, _vp]),
+}
+
 _lock = threading.Lock()
 _lib = None
 
@@ -108,7 +118,7 @@ def load():
                 "CUDA library %s not found: run `python -m litepose_b200.build` "
                 "(there is no CPU/PyTorch fallback for the inference path)" % LIB_PATH)
         lib = ctypes.CDLL(LIB_PATH)
-        for name, (res, args) in SIGNATURES.items():
+        for name, (res, args) in list(SIGNATURES.items()) + list(TRAIN_SIGNATURES.items()):
             fn = getattr(lib, name)   # AttributeError if the .so lacks a declared symbol
             fn.restype = res
             fn.argtypes = args

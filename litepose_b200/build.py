@@ -37,7 +37,7 @@ def _sources():
 def _digest():
     h = hashlib.sha256()
     files = _sources() + [os.path.join(CSRC, f) for f in sorted(os.listdir(CSRC)) if f.endswith(".cuh")]
-    files.append(os.path.join(INCLUDE, "litepose_b200.h"))
+    files += [os.path.join(INCLUDE, f) for f in sorted(os.listdir(INCLUDE)) if f.endswith(".h")]
     for f in files:
         h.update(f.encode())
         with open(f, "rb") as fh:

@@ -11,7 +11,9 @@ shapes and creation order equal the reference's (pose_supermobilenet.py:23-63, l
 ``search_arch`` when ``is_search`` is set).  In eval mode on a CUDA tensor it then runs that sub-network on the sm_90a
 kernels: ``litepose_b200.subnet.derive_supernet_subnet`` applies the supernet's rules (prefix slices, the k = 5 / 3
 depthwise transform, its own strides and identity adds) and a ``LitePoseEngine`` runs the result; engines are cached
-per (device, architecture), a few at a time.  CPU tensors and training mode run the module tree.
+per (device, architecture), a few at a time.  CPU tensors and training mode run the module tree; after
+``litepose_b200.train_dw.convert_depthwise`` its depthwise convolutions, the functional ones of ``SuperSepConv2d`` and
+``SuperInvBottleneck`` included, run on the training kernels for CUDA tensors.
 
 ``lp_recalibrate_bn(x)`` is the search's BN recalibration pass (calibrate_test.py: ``model.train(); model(images)``) on
 the kernels: it does to the module's BatchNorm buffers what a train-mode forward does, without autograd, and returns
@@ -30,6 +32,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from litepose_b200.arch_manager import ArchManager, _make_divisible
+from litepose_b200.train_dw import DepthwiseConv2d
 from ._engine_module import EngineModule, _EngineCache
 from .pose_mobilenet import convbnrelu
 
@@ -79,7 +82,11 @@ class SuperSepConv2d(nn.Module):
     def forward(self, x, num_channel):
         c = x.shape[1]
         dw, pw = self.conv[0], self.conv[3]
-        x = F.conv2d(x, dw.weight[:c], None if dw.bias is None else dw.bias[:c], dw.stride, dw.padding, dw.dilation, c)
+        if isinstance(dw, DepthwiseConv2d):     # convert_depthwise: the training kernels on CUDA tensors
+            x = dw.forward_weight(x, dw.weight[:c])
+        else:
+            x = F.conv2d(x, dw.weight[:c], None if dw.bias is None else dw.bias[:c], dw.stride, dw.padding, dw.dilation,
+                         c)
         x = self.conv[2](self.conv[1](x))
         return F.conv2d(x, pw.weight[:num_channel, :c], None if pw.bias is None else pw.bias[:num_channel],
                         pw.stride, pw.padding, pw.dilation, pw.groups)
@@ -115,8 +122,11 @@ class SuperInvBottleneck(nn.Module):
         lin = {5: self.Linear5x5, 3: self.Linear3x3}.get(ker_size)
         if lin is not None:
             w = lin(w.reshape(w.shape[0], w.shape[1], -1)).reshape(w.shape[0], w.shape[1], ker_size, ker_size)
-        b = None if conv.bias is None else conv.bias[:mid]
-        y = F.conv2d(y, w, b, conv.stride, ker_size // 2, conv.dilation, mid)
+        if isinstance(conv, DepthwiseConv2d):   # convert_depthwise: the training kernels on CUDA tensors
+            y = conv.forward_weight(y, w)
+        else:
+            b = None if conv.bias is None else conv.bias[:mid]
+            y = F.conv2d(y, w, b, conv.stride, ker_size // 2, conv.dilation, mid)
         y = self.depth_conv[2](self.depth_conv[1](y))
         y = self.point_conv[1](self.point_conv[0](y, out_nc))
         return y + x if self.use_residual_connection else y
