@@ -1,5 +1,5 @@
-"""ctypes binding of the C-ABI shared library (include/litepose_b200.h, and include/litepose_b200_train.h for the
-training kernels).
+"""ctypes binding of the C-ABI shared library (include/litepose_b200.h, and include/litepose_b200_train.h and
+include/litepose_b200_train_bn.h for the training kernels).
 
 The CUDA library is the product: there is no Python/PyTorch fallback.  Importing
 this module never compiles anything; ``load()`` raises ``LitePoseLibraryError`` if the
@@ -101,6 +101,13 @@ TRAIN_SIGNATURES = {
     "lp_dw_nchw_wgrad": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _sz, _vp]),
 }
 
+# every symbol declared in include/litepose_b200_train_bn.h (the same library)
+TRAIN_BN_SIGNATURES = {
+    "lp_bn_nchw_workspace_bytes": (_sz, [_i, _i, _i, _i]),
+    "lp_bn_nchw_fwd": (_i, [_vp, _vp, _vp, _vp, _vp, _d, _d, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _sz, _vp]),
+    "lp_bn_nchw_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _sz, _vp]),
+}
+
 _lock = threading.Lock()
 _lib = None
 
@@ -118,7 +125,8 @@ def load():
                 "CUDA library %s not found: run `python -m litepose_b200.build` "
                 "(there is no CPU/PyTorch fallback for the inference path)" % LIB_PATH)
         lib = ctypes.CDLL(LIB_PATH)
-        for name, (res, args) in list(SIGNATURES.items()) + list(TRAIN_SIGNATURES.items()):
+        for name, (res, args) in (list(SIGNATURES.items()) + list(TRAIN_SIGNATURES.items()) +
+                                  list(TRAIN_BN_SIGNATURES.items())):
             fn = getattr(lib, name)   # AttributeError if the .so lacks a declared symbol
             fn.restype = res
             fn.argtypes = args

@@ -7,7 +7,8 @@
 //                     pixels r * BN_ROWS + l + k * RL, k = 0, 1, ... (RL = 256 / VT lanes) in fp64, sum and sum of squares
 //                     from +0; the lanes are then added in lane order 0, 1, ..., RL - 1, starting from lane 0's sums.
 //   bn_stats_merge    one thread per channel adds the CTA partials in pixel-range order r = 0, 1, ..., starting from
-//                     range 0's, then derives in fp64, every operation rounded once (no contraction):
+//                     range 0's, then derives in fp64, every operation rounded once (no contraction), as
+//                     bn_merge_channel (bn_merge.cuh) states:
 //                       mean = S1 / M, var = max(S2 / M - mean * mean, 0), var_unbiased = var * M / (M - 1),
 //                       s = gamma / sqrt(var + eps), scale = fp32(s), shift = fp32(beta - mean * s),
 //                       new running = fp32((1 - momentum) * running + momentum * stat) for (mean, var_unbiased),
@@ -16,7 +17,7 @@
 //
 // lp_bn_apply_f16: y = act(fmaf(x, scale, shift)) (+ residual) in fp32, one rounding to fp16, 8 channels per 16-byte
 // vector.  act: ReLU is (v > 0 ? v : +0), ReLU6 then (v < 6 ? v : 6); y may alias x.
-#include "common.cuh"
+#include "bn_merge.cuh"
 
 namespace lp {
 
@@ -105,28 +106,12 @@ bn_stats_merge(const double* __restrict__ part, int nparts, long long M, int C, 
                float* __restrict__ new_mean, float* __restrict__ new_var, int* __restrict__ nonfinite) {
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= C) return;
-    double t1 = part[2 * c], t2 = part[2 * c + 1];
-    for (int i = 1; i < nparts; ++i) {
-        const size_t o = (size_t)i * C + c;
-        t1 = __dadd_rn(t1, part[2 * o]);
-        t2 = __dadd_rn(t2, part[2 * o + 1]);
-    }
-    const double m = (double)M;
-    const double mean = __ddiv_rn(t1, m);
-    double var = __dsub_rn(__ddiv_rn(t2, m), __dmul_rn(mean, mean));
-    var = var > 0.0 ? var : 0.0;
-    const double var_u = __ddiv_rn(__dmul_rn(var, m), __dsub_rn(m, 1.0));
-    const double s = __ddiv_rn((double)gamma[c], __dsqrt_rn(__dadd_rn(var, eps)));
-    const float sc = __double2float_rn(s);
-    const float sh = __double2float_rn(__dsub_rn((double)beta[c], __dmul_rn(mean, s)));
-    const double keep = __dsub_rn(1.0, momentum);
-    const float nm = __double2float_rn(__dadd_rn(__dmul_rn(keep, (double)rmean[c]), __dmul_rn(momentum, mean)));
-    const float nv = __double2float_rn(__dadd_rn(__dmul_rn(keep, (double)rvar[c]), __dmul_rn(momentum, var_u)));
-    scale[c] = sc;
-    shift[c] = sh;
-    new_mean[c] = nm;
-    new_var[c] = nv;
-    if (!(isfinite(sc) && isfinite(sh) && isfinite(nm) && isfinite(nv))) *nonfinite = 1;
+    const BnMerged r = bn_merge_channel(part, nparts, M, C, c, gamma[c], beta[c], rmean[c], rvar[c], momentum, eps);
+    scale[c] = r.scale;
+    shift[c] = r.shift;
+    new_mean[c] = r.new_mean;
+    new_var[c] = r.new_var;
+    if (!(isfinite(r.scale) && isfinite(r.shift) && isfinite(r.new_mean) && isfinite(r.new_var))) *nonfinite = 1;
 }
 
 template <int ACT>

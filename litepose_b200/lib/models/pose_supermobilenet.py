@@ -321,10 +321,11 @@ class SuperLitePose(EngineModule):
     @staticmethod
     def _permute_bn(bn, idx):
         """weight and bias only: the reference moves the running statistics for modules whose type is exactly
-        BatchNorm1d / BatchNorm2d, which no SuperBatchNorm2d is"""
+        BatchNorm1d / BatchNorm2d, which no SuperBatchNorm2d is.  A module converted by
+        litepose_b200.train_bn.convert_batchnorm counts as the class it was converted from (``lp_base``)."""
         bn.weight.data = torch.index_select(bn.weight.data, 0, idx)
         bn.bias.data = torch.index_select(bn.bias.data, 0, idx)
-        if type(bn) in (nn.BatchNorm1d, nn.BatchNorm2d):
+        if getattr(type(bn), "lp_base", type(bn)) in (nn.BatchNorm1d, nn.BatchNorm2d):
             bn.running_mean.data = torch.index_select(bn.running_mean.data, 0, idx)
             bn.running_var.data = torch.index_select(bn.running_var.data, 0, idx)
 
