@@ -104,6 +104,8 @@ int lp_dwconv_f16(const void* x, const void* w, const float* bias, void* y, int 
  * building engines / capturing graphs. */
 void lp_set_dw_precision(int prec);
 int lp_get_dw_precision(void);
+/* The SM limit the persistent kernels size their grids from (a test and debug seam) is declared in
+ * include/litepose_b200_debug.h. */
 
 /* ---- M1/M2: pointwise 1x1 as a wgmma GEMM ---------------------------------
  * out[M,N] = act(a[M,K] * W^T + bias) (+ residual[M,N]);  a/out/residual fp16 row-major

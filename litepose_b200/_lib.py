@@ -1,5 +1,5 @@
 """ctypes binding of the C-ABI shared library (include/litepose_b200.h, and include/litepose_b200_train.h and
-include/litepose_b200_train_bn.h for the training kernels).
+include/litepose_b200_train_bn.h for the training kernels, include/litepose_b200_debug.h for the SM limit).
 
 The CUDA library is the product: there is no Python/PyTorch fallback.  Importing
 this module never compiles anything; ``load()`` raises ``LitePoseLibraryError`` if the
@@ -108,6 +108,13 @@ TRAIN_BN_SIGNATURES = {
     "lp_bn_nchw_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _sz, _vp]),
 }
 
+# every symbol declared in include/litepose_b200_debug.h (the same library): library state for tests and debugging,
+# launching nothing
+DEBUG_SIGNATURES = {
+    "lp_set_sm_limit": (None, [_i]),
+    "lp_get_sm_limit": (_i, []),
+}
+
 _lock = threading.Lock()
 _lib = None
 
@@ -126,7 +133,7 @@ def load():
                 "(there is no CPU/PyTorch fallback for the inference path)" % LIB_PATH)
         lib = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in (list(SIGNATURES.items()) + list(TRAIN_SIGNATURES.items()) +
-                                  list(TRAIN_BN_SIGNATURES.items())):
+                                  list(TRAIN_BN_SIGNATURES.items()) + list(DEBUG_SIGNATURES.items())):
             fn = getattr(lib, name)   # AttributeError if the .so lacks a declared symbol
             fn.restype = res
             fn.argtypes = args

@@ -1,4 +1,4 @@
-// Library state of the C ABI: thread-local error string, launch counter, device check,
+// Library state of the C ABI: thread-local error string, launch counter, device check, SM count and its limit,
 // tensor-map construction through the driver entry point (no link-time libcuda dependency).
 #include <atomic>
 #include <cstdarg>
@@ -6,6 +6,7 @@
 #include <mutex>
 
 #include "common.cuh"
+#include "../../include/litepose_b200_debug.h"
 
 namespace lp {
 
@@ -117,18 +118,25 @@ int make_tmap_taps(CUtensorMap* map, const void* w, int taps, int C) {
     return make_tmap(map, w, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE);
 }
 
+// lp_set_sm_limit: 0 = no limit.  Process-wide, so a pipeline's worker threads size their grids from the same count.
+static std::atomic<int> g_sm_limit{0};
+
 int num_sms() {
     static thread_local int cached_dev = -1;
     static thread_local int cached = 0;
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
-    if (dev != cached_dev) {
-        int v = 0;
-        if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;
-        cached = v;
-        cached_dev = dev;
+    int v = 132;
+    if (cudaGetDevice(&dev) == cudaSuccess) {
+        if (dev != cached_dev) {
+            int a = 0;
+            if (cudaDeviceGetAttribute(&a, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || a <= 0) a = 132;
+            cached = a;
+            cached_dev = dev;
+        }
+        v = cached;
     }
-    return cached;
+    const int limit = g_sm_limit.load(std::memory_order_relaxed);
+    return limit > 0 && limit < v ? limit : v;
 }
 
 }  // namespace lp
@@ -153,3 +161,6 @@ extern "C" int lp_device_check(void) {
 
 extern "C" uint64_t lp_launch_count(void) { return lp::g_launches.load(); }
 extern "C" void lp_reset_launch_count(void) { lp::g_launches.store(0); }
+
+extern "C" void lp_set_sm_limit(int n) { lp::g_sm_limit.store(n > 0 ? n : 0, std::memory_order_relaxed); }
+extern "C" int lp_get_sm_limit(void) { return lp::num_sms(); }
